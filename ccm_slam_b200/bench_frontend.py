@@ -93,4 +93,110 @@ def run(oracle=None, reps=30, cpu_reps=3):
         out["parity"] = {"orb_bit_exact": bool(len(rk) == len(k1) and np.array_equal(rd, d1) and np.array_equal(rk["x"], k1["x"])),
                          "bow_indices_equal": bool(rn == n_b and np.array_equal(ref_b, got_b)),
                          "triangulation_indices_equal": bool(np.array_equal(ref_t, got_t))}
+    kb = kfdb_block(oracle, reps)
+    parity = kb.pop("parity", {})
+    out.update(kb)
+    if parity:
+        out.setdefault("parity", {}).update(parity)
+    return out
+
+
+def _spread(ts):
+    q = np.percentile(ts, [10, 50, 90])
+    return dict(p10=float(q[0]), median=float(q[1]), p90=float(q[2]), n=len(ts))
+
+
+def _card():
+    import subprocess
+    name, plim = None, None
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"], capture_output=True,
+                           text=True, timeout=20)
+        name, plim = [x.strip() for x in r.stdout.strip().splitlines()[0].split(",")]
+    except Exception:
+        pass
+    return name, plim
+
+
+def kfdb_block(oracle=None, reps=30):
+    """DetectLoopCandidates on a server-shaped database (4 agents x 2500 keyframes, ~660 words each, 200 k-word vocabulary): one
+    query per call (ccm_kfdb_query + ccm_kfdb_select, host buffers), a batch of 64 queries, CUDA-event time of the kernels, and the
+    CPU oracle port of S/Database.cpp on the same database."""
+    import importlib
+    from . import synth_match as sm
+    from .frontend import KeyFrameDatabase
+    d = sm.make_place_db(n_clients=4, kf_per_client=2500, n_words=200000, local_words=400, bg_words=150, pool=1200, seed=5)
+    K = len(d["uid"])
+    idx = {int(u): k for k, u in enumerate(d["uid"])}
+    covis = lambda u: sm.place_db_covis(d, idx[int(u)])
+    db = KeyFrameDatabase(d["n_words"], 0)
+    for k in range(K):
+        db.add(d["uid"][k], d["client"][k], *sm.place_db_bow(d, k))
+    rows = [K - 1 - i for i in range(64)]
+    reqs, mins, info = [], [], []
+    for k in rows:
+        w, v = sm.place_db_bow(d, k)
+        nb = sm.place_db_covis(d, k)
+        ms = float(np.float32(db.score_many(w, v, nb).min()) * np.float32(0.8)) if len(nb) else 0.0   # LoopFinder.cpp:125-142
+        reqs.append(db.request(w, v, 1 << int(d["client"][k]), np.concatenate([[d["uid"][k]], nb]).astype(np.uint64)))
+        mins.append(ms); info.append((int(d["uid"][k]), nb))
+    i = [0]
+
+    def one():
+        j = i[0] % len(reqs); i[0] += 1
+        return db.select(db.query_batch([reqs[j]])[0], covis, False, mins[j])
+    for _ in range(5):
+        one()
+    ts = []
+    for _ in range(max(reps, 50)):
+        t0 = time.perf_counter(); one(); ts.append((time.perf_counter() - t0) * 1e3)
+    out = {"kfdb_query_ms_per_call": statistics.median(ts), "kfdb_query_ms_spread": _spread(ts)}
+    db.query_batch(reqs)
+    tb = []
+    for _ in range(10):
+        t0 = time.perf_counter()
+        res = db.query_batch(reqs)
+        for r, ms in zip(res, mins):
+            db.select(r, covis, False, ms)
+        tb.append((time.perf_counter() - t0) * 1e3 / len(reqs))
+    out["kfdb_query_batch_ms_per_query"] = statistics.median(tb)
+    out["kfdb_query_batch_spread"] = _spread(tb)
+    out["kfdb_batch"] = len(reqs)
+    db.set_timing(True)
+    for _ in range(3):
+        db.query_batch([reqs[0]])
+    tc, tsc, nq = db.timing()
+    db.set_timing(True)
+    db.query_batch(reqs)
+    bc, bsc, bn = db.timing()
+    db.set_timing(False)
+    out["kfdb_kernel_ms_per_query"] = {"count": tc / nq, "score": tsc / nq, "batch64_count": bc / bn, "batch64_score": bsc / bn}
+    first = db.query_batch([reqs[0]])[0]
+    out["kfdb_database"] = {"keyframes": K, "clients": 4, "postings": int(len(d["bow_word"])), "vocabulary": d["n_words"],
+                            "query_candidates_scored": int(len(first["cand"])), "query_sharing": int(first["n_sharing"])}
+    name, plim = _card()
+    out["kfdb_card"] = {"name": name, "power_limit": plim}
+    if oracle is not None:
+        pk = importlib.import_module(oracle.__name__.rsplit(".", 1)[0] + ".pykfdb")
+        o = pk.Oracle(d["n_words"], 0)
+        for k in range(K):
+            o.keyframe(d["uid"][k], d["client"][k], *sm.place_db_bow(d, k))
+            o.set_covis(d["uid"][k], sm.place_db_covis(d, k))
+        for k in range(K):
+            o.add(d["uid"][k])
+        by_client = {c: d["uid"][d["client"] == c] for c in range(4)}
+        equal = True
+        tc = []
+        for j, k in enumerate(rows[:16]):
+            uid, nb = info[j]
+            t0 = time.perf_counter()
+            want = o.DetectLoopCandidates(uid, mins[j], nb, by_client[int(d["client"][k])])
+            tc.append((time.perf_counter() - t0) * 1e3)
+            got = db.select(db.query_batch([reqs[j]])[0], covis, False, mins[j])
+            equal = equal and got.tolist() == want.tolist()
+        out["cpu_kfdb_query_ms_per_call"] = statistics.median(tc)
+        out["cpu_kfdb_query_ms_spread"] = _spread(tc)
+        out.setdefault("parity", {})["kfdb_candidates_equal"] = bool(equal)
+        o.close()
+    db.close()
     return out

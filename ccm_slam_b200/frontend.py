@@ -419,3 +419,143 @@ class KeyFrameStore:
             self.close()
         except Exception:
             pass
+
+
+class KfdbRequestC(C.Structure):
+    _fields_ = [("n", C.c_int32), ("word", C.c_void_p), ("value", C.c_void_p), ("client_mask", C.c_uint64), ("n_exclude", C.c_int32),
+                ("exclude_uid", C.c_void_p)]
+
+
+class KfdbResultC(C.Structure):
+    _fields_ = [("cand", C.c_void_p), ("cap", C.c_int32), ("n", C.c_int32), ("n_sharing", C.c_int32), ("max_common", C.c_int32),
+                ("min_common", C.c_int32)]
+
+
+KFDB_CAND_DTYPE = np.dtype([("uid", "<u8"), ("n_words", "<i4"), ("score", "<f4"), ("score_f64", "<f8")])   # ccm_kfdb_candidate
+ALL_CLIENTS = (1 << 64) - 1
+
+
+class KeyFrameDatabase:
+    """cslam::KeyFrameDatabase (I/Database.h, S/Database.cpp) with the inverted file and the BowVectors on the device.
+    Keyframes are named by uid = mUniqueId and carry client = mId.second; a BowVector is (word ids ascending, values).
+
+      add / erase / clear                          S/Database.cpp:37-70
+      DetectLoopCandidates / DetectMapMatchCandidates / DetectRelocalizationCandidates   :72-439
+      query / query_batch                          the device half alone: the scored candidates in the reference's order
+      score_many                                   mpVoc->score(query, keyframe) for a list of resident keyframes
+
+    `covis` (the Detect* methods) maps a uid to its GetBestCovisibilityKeyFrames(10) (a dict or a callable); it is read for the
+    scored candidates only.  `last_result` holds the device result (the scored candidates) of the last Detect* call."""
+
+    def __init__(self, n_words, scoring=0):
+        L = lib()
+        L.ccm_kfdb_size.restype = C.c_int64
+        L.ccm_kfdb_size.argtypes = [C.c_void_p]
+        L.ccm_kfdb_destroy.argtypes = [C.c_void_p]
+        L.ccm_kfdb_add.argtypes = [C.c_void_p, C.c_uint64, C.c_uint32, C.c_int32, C.c_void_p, C.c_void_p]
+        L.ccm_kfdb_erase.argtypes = [C.c_void_p, C.c_uint64]
+        L.ccm_kfdb_select.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_float, C.c_void_p, C.c_void_p]
+        self._h = C.c_void_p()
+        self.n_words, self.scoring = int(n_words), int(scoring)
+        _chk(L.ccm_kfdb_create(self.n_words, self.scoring, C.byref(self._h)))
+        self.client_of = {}
+        self.last_result = None
+
+    def close(self):
+        if self._h:
+            lib().ccm_kfdb_destroy(self._h)
+            self._h = C.c_void_p()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def add(self, uid, client, word, value):
+        w = np.ascontiguousarray(word, np.uint32); v = np.ascontiguousarray(value, np.float64)
+        _chk(lib().ccm_kfdb_add(self._h, int(uid), int(client), len(w), _p(w), _p(v)))
+        self.client_of[int(uid)] = int(client)
+
+    def erase(self, uid):
+        _chk(lib().ccm_kfdb_erase(self._h, int(uid)))
+        self.client_of.pop(int(uid), None)
+
+    def clear(self):
+        _chk(lib().ccm_kfdb_clear(self._h))
+        self.client_of.clear()
+
+    def size(self):
+        return lib().ccm_kfdb_size(self._h)
+
+    def score_many(self, word, value, uids):
+        w = np.ascontiguousarray(word, np.uint32); v = np.ascontiguousarray(value, np.float64); u = np.ascontiguousarray(uids, np.uint64)
+        out = np.zeros(len(u))
+        _chk(lib().ccm_kfdb_score_many(self._h, len(w), _p(w), _p(v), len(u), _p(u), _p(out)))
+        return out
+
+    @staticmethod
+    def request(word, value, client_mask=ALL_CLIENTS, exclude=()):
+        """one query: (word, value) = its BowVector; keyframes of clients outside client_mask and the uids in exclude are invisible"""
+        keep = dict(w=np.ascontiguousarray(word, np.uint32), v=np.ascontiguousarray(value, np.float64),
+                    x=np.ascontiguousarray(list(exclude) if not isinstance(exclude, np.ndarray) else exclude, np.uint64))
+        return KfdbRequestC(len(keep["w"]), _p(keep["w"]), _p(keep["v"]), int(client_mask) & ALL_CLIENTS, len(keep["x"]), _p(keep["x"])), keep
+
+    def query_batch(self, requests):
+        """requests: list of request() tuples -> list of dict(cand = KFDB_CAND_DTYPE array, n_sharing, max_common, min_common)"""
+        nq = len(requests)
+        cap = max(1, self.size())
+        Q = (KfdbRequestC * max(nq, 1))(*[r[0] for r in requests])
+        cands = [np.zeros(cap, KFDB_CAND_DTYPE) for _ in range(nq)]
+        R = (KfdbResultC * max(nq, 1))(*[KfdbResultC(_p(c), cap, 0, 0, 0, 0) for c in cands])
+        _chk(lib().ccm_kfdb_query_batch(self._h, Q, nq, R))
+        return [dict(cand=cands[b][:R[b].n].copy(), n_sharing=R[b].n_sharing, max_common=R[b].max_common, min_common=R[b].min_common,
+                     _res=R[b]) for b in range(nq)]
+
+    def query(self, word, value, client_mask=ALL_CLIENTS, exclude=()):
+        return self.query_batch([self.request(word, value, client_mask, exclude)])[0]
+
+    @staticmethod
+    def select(result, covis, reloc=False, min_score=0.0):
+        """ccm_kfdb_select (host only): covisibility accumulation and retain over a query result -> uids of the returned vector<kfptr>"""
+        cand = np.ascontiguousarray(result["cand"])
+        get = covis if callable(covis) else (lambda u: covis.get(int(u), ()))
+        lists = [np.asarray(get(u), np.uint64) for u in cand["uid"]]
+        ptr = np.concatenate([[0], np.cumsum([len(x) for x in lists])]).astype(np.int32)
+        cu = np.concatenate(lists).astype(np.uint64) if lists else np.zeros(0, np.uint64)
+        res = KfdbResultC(_p(cand), len(cand), len(cand), result["n_sharing"], result["max_common"], result["min_common"])
+        out = np.zeros(max(1, len(cand)), np.uint64); n = C.c_int32()
+        _chk(lib().ccm_kfdb_select(C.byref(res), _p(ptr), _p(cu), int(bool(reloc)), C.c_float(min_score), _p(out), C.byref(n)))
+        return out[:n.value].copy()
+
+    def _mask(self, clients):
+        m = 0
+        for c in clients:
+            m |= 1 << int(c)
+        return m
+
+    def DetectLoopCandidates(self, q_uid, word, value, min_score, connected, in_map, covis):
+        """pKF = (q_uid, BowVector); connected = GetConnectedKeyFrames(); in_map = the uids of GetMapptr()->GetMmpKeyFrames()"""
+        in_map = set(int(u) for u in in_map)
+        clients = {self.client_of[u] for u in in_map if u in self.client_of}
+        hide = {int(q_uid)} | {int(u) for u in connected}
+        hide |= {u for u, c in self.client_of.items() if c in clients and u not in in_map}   # in the database, not in the map
+        r = self.last_result = self.query(word, value, self._mask(clients), sorted(hide))
+        return self.select(r, covis, False, min_score)
+
+    def DetectMapMatchCandidates(self, word, value, min_score, assoc_clients, covis):
+        """pMap->msuAssClients = assoc_clients"""
+        r = self.last_result = self.query(word, value, ALL_CLIENTS & ~self._mask(assoc_clients))
+        return self.select(r, covis, False, min_score)
+
+    def DetectRelocalizationCandidates(self, word, value, covis):
+        r = self.last_result = self.query(word, value)
+        return self.select(r, covis, True)
+
+    def set_timing(self, on=True):
+        _chk(lib().ccm_kfdb_set_timing(self._h, int(bool(on))))
+
+    def timing(self):
+        a = C.c_double(); b = C.c_double(); n = C.c_int64()
+        _chk(lib().ccm_kfdb_get_timing(self._h, C.byref(a), C.byref(b), C.byref(n)))
+        return a.value, b.value, n.value

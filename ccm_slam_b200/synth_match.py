@@ -140,3 +140,70 @@ def make_init_pair(n=1000, seed=0, window=100.0, shift=(6.0, -4.0)):
     q = dict(valid=np.ones(n, np.uint8), uv=g1["kp_xy"].copy(), radius=np.full(n, window, np.float32), level=g1["octave"].copy(),
              desc=g1["desc"], angle=g1["angle"])
     return g2, q
+
+
+def make_place_db(n_clients=4, kf_per_client=60, n_words=20000, local_words=160, bg_words=60, pool=400, revisit=0.3, cross=0.3,
+                  n_dups=4, seed=0):
+    """A server-shaped keyframe database with BowVectors synthesised directly (no vocabulary tree): `n_clients` agents walk along
+    trajectories of places; a keyframe draws `local_words` words from its place's pool (and its neighbour's) and `bg_words` from a
+    Zipf background over the whole vocabulary, so that common words have long inverted lists.  A fraction `revisit` of each
+    trajectory returns to the agent's earlier places (loop candidates) and a fraction `cross` visits another agent's places
+    (map-match candidates).  `n_dups` keyframes copy another keyframe's BowVector exactly: equal scores, ties in the accumulation.
+    Covisibility top-10 lists (GetBestCovisibilityKeyFrames(10)) rank the keyframes of the same agent within 8 steps by shared
+    words (ties: older first).  Values are L1-normalised.
+    Returns dict(n_words, uid, client, place, bow_ptr, bow_word, bow_val, covis_ptr, covis_uid) with uid = mUniqueId (1-based,
+    agents interleaved in time as the server receives them)."""
+    rng = np.random.default_rng(seed)
+    n_places = max(4, kf_per_client // 3)
+    pools = [rng.choice(n_words, size=pool, replace=False) for _ in range(n_clients * n_places)]
+    zipf = 1.0 / np.arange(1, n_words + 1) ** 1.1
+    zipf /= zipf.sum()
+    zperm = rng.permutation(n_words)
+    place_of = []
+    for c in range(n_clients):
+        t = np.minimum(np.arange(kf_per_client) // 3, n_places - 1) + c * n_places
+        for i in range(kf_per_client):
+            u = rng.random()
+            if i > 6 and u < revisit:
+                t[i] = t[rng.integers(0, i - 5)]
+            elif u < revisit + cross:
+                t[i] = rng.integers(0, n_clients * n_places)
+        place_of.append(t)
+    K = n_clients * kf_per_client
+    order = np.arange(K).reshape(n_clients, kf_per_client).T.reshape(-1)      # time-interleaved arrival
+    uid = np.arange(1, K + 1, dtype=np.uint64)
+    client = (order // kf_per_client).astype(np.uint32)
+    place = np.array([place_of[c][i] for c, i in zip(order // kf_per_client, order % kf_per_client)], np.int64)
+    bows = []
+    for k in range(K):
+        p = place[k]
+        loc = rng.choice(pools[p], size=local_words, replace=False)
+        nb = rng.choice(pools[min(p + 1, len(pools) - 1)], size=local_words // 4, replace=False)
+        bg = zperm[rng.choice(n_words, size=bg_words, p=zipf)]
+        w = np.unique(np.concatenate([loc, nb, bg])).astype(np.uint32)
+        v = rng.uniform(0.2, 3.0, len(w))
+        bows.append((w, v / np.abs(v).sum()))
+    for j in range(n_dups):                                                      # exact copies -> equal scores
+        a, b = rng.choice(K, size=2, replace=False)
+        bows[b] = (bows[a][0].copy(), bows[a][1].copy())
+    covis = []
+    sets = [set(w.tolist()) for w, _ in bows]
+    for k in range(K):
+        same = [j for j in range(max(0, k - 8 * n_clients), min(K, k + 8 * n_clients + 1)) if j != k and client[j] == client[k]]
+        same.sort(key=lambda j: (-len(sets[k] & sets[j]), j))
+        covis.append(uid[same[:10]])
+    bow_ptr = np.concatenate([[0], np.cumsum([len(w) for w, _ in bows])]).astype(np.int64)
+    covis_ptr = np.concatenate([[0], np.cumsum([len(c) for c in covis])]).astype(np.int64)
+    return dict(n_words=n_words, uid=uid, client=client, place=place, bow_ptr=bow_ptr,
+                bow_word=np.concatenate([w for w, _ in bows]).astype(np.uint32), bow_val=np.concatenate([v for _, v in bows]),
+                covis_ptr=covis_ptr, covis_uid=np.concatenate(covis).astype(np.uint64) if K else np.zeros(0, np.uint64))
+
+
+def place_db_bow(db, k):
+    """BowVector (word, value) of keyframe row k of make_place_db()"""
+    a, b = db["bow_ptr"][k], db["bow_ptr"][k + 1]
+    return db["bow_word"][a:b], db["bow_val"][a:b]
+
+
+def place_db_covis(db, k):
+    return db["covis_uid"][db["covis_ptr"][k]:db["covis_ptr"][k + 1]]

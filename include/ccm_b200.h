@@ -530,6 +530,71 @@ int ccm_kfstore_transform(ccm_kf_store* s, uint64_t uid, ccm_voc_handle* voc, in
 /* host only (usable without a device): n wire keypoints -> ccm_keypoint, the arithmetic of Converter::fromCvKeyPointMsg */
 int ccm_wire_keypoints_decode(const uint8_t* keypoints_wire, int32_t n, ccm_keypoint* out);
 
+/* ---- device-resident keyframe database (place recognition) --------------------------------------------------------
+ * Replaces cslam::KeyFrameDatabase (cslam/src/Database.cpp): add :37-43, erase :45-64, clear :66-70 and the candidate
+ * queries DetectLoopCandidates :72-202, DetectMapMatchCandidates :204-327, DetectRelocalizationCandidates :329-439 with the
+ * DBoW2 scores they call (thirdparty/DBoW2/DBoW2/ScoringObject.cpp:23-311).  One database serves every agent and map of the
+ * server (cslam/src/server/ServerSystem.cpp:185).  uid = mUniqueId, client = mId.second; a BowVector is (n, word[], value[]) in
+ * std::map order.  The inverted file and the BowVectors live on the device; within a word the postings keep the reference's
+ * list order (insertion order minus erased entries).
+ * A query counts shared words per visible keyframe, keeps those with more than minCommonWords = (int)(max * 0.8f) and scores
+ * them against the query: the output is the reference's scored list (lScoreAndMatch before the minScore filter) in the order
+ * of lKFsSharingWords.  A keyframe is visible when its client's bit is set in client_mask and its uid is not in exclude_uid:
+ *   DetectLoopCandidates      mask = the clients of the query's map; exclude = the query keyframe, GetConnectedKeyFrames(), and
+ *                             every database keyframe of those clients that is not in GetMapptr()->GetMmpKeyFrames()
+ *   DetectMapMatchCandidates  mask = every client not in pMap->msuAssClients; exclude = none
+ *   DetectRelocalizationCandidates  mask = all ones; exclude = none
+ * ccm_kfdb_select then runs the covisibility accumulation and the 0.75 * bestAccScore retain on the host.
+ * Thread-safe per handle; every call returns after its device work has finished. */
+typedef struct ccm_kfdb ccm_kfdb;
+typedef struct ccm_kfdb_request {
+  int32_t n;                 /* the query's BowVector */
+  const uint32_t* word;      /* n, strictly ascending */
+  const double* value;       /* n */
+  uint64_t client_mask;      /* bit c: keyframes of client c are visible (client ids < 64) */
+  int32_t n_exclude;
+  const uint64_t* exclude_uid; /* n_exclude uids that are invisible (uids not in the database are ignored) */
+} ccm_kfdb_request;
+typedef struct ccm_kfdb_candidate {
+  uint64_t uid;
+  int32_t n_words;           /* shared words (mnLoopWords / mnRelocWords) */
+  float score;               /* (float) of the score: what mLoopScore / mRelocScore receive */
+  double score_f64;          /* mpVoc->score(query, keyframe) */
+} ccm_kfdb_candidate;
+typedef struct ccm_kfdb_result {
+  ccm_kfdb_candidate* cand;  /* caller-allocated, cap entries (ccm_kfdb_size is always enough) */
+  int32_t cap;
+  int32_t n;                 /* scored candidates, in the reference's order */
+  int32_t n_sharing;         /* visible keyframes sharing at least one word (lKFsSharingWords.size()) */
+  int32_t max_common, min_common;
+} ccm_kfdb_result;
+int ccm_kfdb_create(int32_t n_words /*vocabulary size*/, int32_t scoring /*DBoW2::ScoringType*/, ccm_kfdb** out);
+void ccm_kfdb_destroy(ccm_kfdb* h);
+/* a keyframe already in the database is refused (erase it first); erasing an unknown uid is a no-op */
+int ccm_kfdb_add(ccm_kfdb* h, uint64_t uid, uint32_t client, int32_t n, const uint32_t* word, const double* value);
+int ccm_kfdb_erase(ccm_kfdb* h, uint64_t uid);
+int ccm_kfdb_clear(ccm_kfdb* h);
+int64_t ccm_kfdb_size(ccm_kfdb* h);       /* keyframes in the database, -1 for a null handle */
+int ccm_kfdb_query(ccm_kfdb* h, const ccm_kfdb_request* q, ccm_kfdb_result* r);
+/* nq queries against the same database state in one launch sequence; identical to nq calls of ccm_kfdb_query */
+int ccm_kfdb_query_batch(ccm_kfdb* h, const ccm_kfdb_request* q, int32_t nq, ccm_kfdb_result* r);
+/* score[i] = mpVoc->score(query, keyframe uid[i]) (the minScore loop over the covisible keyframes, LoopFinder.cpp:125-139) */
+int ccm_kfdb_score_many(ccm_kfdb* h, int32_t n, const uint32_t* word, const double* value, int32_t n_uid, const uint64_t* uid,
+                        double* score);
+/* CUDA-event time of the counting kernels and of the threshold / order / score kernels, summed over queries while on */
+int ccm_kfdb_set_timing(ccm_kfdb* h, int32_t on);   /* also zeroes the sums */
+int ccm_kfdb_get_timing(ccm_kfdb* h, double* count_ms, double* score_ms, int64_t* queries);
+/* host only (usable without a device): candidate r->cand[i]'s GetBestCovisibilityKeyFrames(10) is covis_uid[covis_ptr[i] ..
+ * covis_ptr[i+1]), in its order.  reloc = 0: loop / map-match (minScore filter, bestAccScore starts at min_score); reloc = 1:
+ * relocalisation (no filter, bestAccScore starts at 0).  out_uid (r->n entries) receives the returned vector<kfptr>.
+ * Equivalence with the reference: the queries are stateless, Database.cpp reads marker members left by earlier queries.  They agree
+ * whenever each (kind, query id) is queried once (LoopFinder, MapMatcher, Tracking) and, for relocalisation, whenever the mRelocScore
+ * of every covisible keyframe that shares a word with the frame but is not scored in this query is 0: the reference adds that value
+ * (Database.cpp:403-406 checks mRelocQuery only), left by an earlier relocalisation query or uninitialised; this selection adds
+ * nothing for such a keyframe, and the ABI has no input that would reproduce the stale value (DESIGN.md §5). */
+int ccm_kfdb_select(const ccm_kfdb_result* r, const int32_t* covis_ptr, const uint64_t* covis_uid, int32_t reloc, float min_score,
+                    uint64_t* out_uid, int32_t* n_out);
+
 #ifdef __cplusplus
 }
 #endif
