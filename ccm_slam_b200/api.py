@@ -5,6 +5,7 @@ if the library is missing, or no CUDA device is present, the calls raise.
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 import os
 
@@ -261,6 +262,23 @@ class BAHandle:
         _chk(lib().ccm_ba_debug_schur(self._h, int(robust), C.c_double(huber_delta), C.c_double(lam), _p(S), _p(bs), _p(dxp), _p(dxl), C.byref(it), C.byref(rr)))
         return dict(S=S, bschur=bs, dx_pose=dxp, dx_point=dxl, pcg_iters=it.value, pcg_relres=rr.value)
 
+    def debug_schur_blocks(self):
+        """S and b_schur as the last debug_schur left them: block CSR in pose indices (rowptr (K+1,), col (nnzb,), val (nnzb,6,6)),
+        fixed poses with empty rows, and b_schur (K,6)."""
+        nnzb = self.info()["s_blocks_full"]
+        rowptr = np.empty(self.K + 1, np.int32); col = np.empty(max(nnzb, 1), np.int32); val = np.empty((max(nnzb, 1), 6, 6))
+        bs = np.empty((self.K, 6))
+        _chk(lib().ccm_ba_debug_schur_blocks(self._h, _p(rowptr), _p(col), _p(val), _p(bs)))
+        return dict(rowptr=rowptr, col=col[:nnzb], val=val[:nnzb], bschur=bs)
+
+    PATH_KEYS = ("schur_mode", "panels_on", "panels", "covered", "pcg_impl", "pcg_block", "pcg_agg", "pcg_nc")
+
+    def debug_paths(self):
+        """what the handle runs: Schur mode in effect, panels, PCG kernel, CTA size and coarse space"""
+        out = np.zeros(8, np.int32)
+        _chk(lib().ccm_ba_debug_paths(self._h, _p(out)))
+        return {k: int(v) for k, v in zip(self.PATH_KEYS, out)}
+
     def set_estimate(self, poses=None, points=None):
         """replace the estimate, keep structure and observations on the device (ccm_ba_set_estimate)"""
         ps = None if poses is None else np.ascontiguousarray(poses, np.float64)
@@ -277,6 +295,17 @@ class BAHandle:
         ms = C.c_double()
         _chk(lib().ccm_ba_time_kernel(self._h, which, reps, C.c_double(huber_delta), C.c_double(lam), C.byref(ms)))
         return ms.value
+
+
+@contextlib.contextmanager
+def schur_mode(mode: int):
+    """ccm_ba_debug_set_schur_mode for the duration of a block.  The override is process-global, so it is always put back to -1
+    (the CCM_SCHUR environment variable / built-in default), also when the block raises."""
+    _chk(lib().ccm_ba_debug_set_schur_mode(int(mode)))
+    try:
+        yield
+    finally:
+        _chk(lib().ccm_ba_debug_set_schur_mode(-1))
 
 
 def poses_from_Tcw_f32(T):

@@ -329,9 +329,10 @@ __global__ void __launch_bounds__(TPB) k_schur(const uint2* __restrict__ prod, c
                                                const int* __restrict__ u_row, const int* __restrict__ u_col, int nub,
                                                const double* __restrict__ Z, const int* __restrict__ o_lm,
                                                const double* __restrict__ gvec, double* __restrict__ U_val,
-                                               double* __restrict__ bneg) {
+                                               double* __restrict__ bneg, const unsigned char* __restrict__ covered = nullptr) {
   const int warp = (int)(((long long)blockIdx.x * TPB + threadIdx.x) >> 5);
   if (warp >= nub) return;
+  if (covered != nullptr && covered[warp]) return;  // this block belongs to the panel kernel (schur_panel.cuh)
   const int lane = threadIdx.x & 31;
   const int r = lane % 6, s = lane / 6;  // lanes 30,31: s == 5 -> idle stream
   const unsigned beg = u_prod_ptr[warp], end = u_prod_ptr[warp + 1];
@@ -621,11 +622,13 @@ constexpr int RS_SHIFT = 13;
 template <int UNROLL>
 __global__ void __launch_bounds__(32 * RS_W) k_schur_rowsync(const uint2* __restrict__ prod, const unsigned* __restrict__ u_prod_ptr,
                                                              const int* __restrict__ rs_first, const int* __restrict__ rs_count,
-                                                             const double* __restrict__ Z, double* __restrict__ U_val) {
+                                                             const double* __restrict__ Z, double* __restrict__ U_val,
+                                                             const unsigned char* __restrict__ covered = nullptr) {
   __shared__ unsigned s_cmin, s_cmax;
   const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int count = rs_count[blockIdx.x];
-  const bool active = w < count;
+  // a block the panel kernel owns (schur_panel.cuh) has an empty list here and must not be overwritten; its warp still takes the barriers
+  const bool active = w < count && !(covered != nullptr && covered[rs_first[blockIdx.x] + w]);
   const int u = active ? rs_first[blockIdx.x] + w : 0;
   const int m = lane >> 2, k = lane & 3;
   const bool ld = m < 6 && k < 3;

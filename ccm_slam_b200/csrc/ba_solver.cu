@@ -276,7 +276,8 @@ int schur_mode() {
 template <int UNROLL, int CTA>
 void launch_schur_tiled(ccm_ba_handle* h, cudaStream_t s) {
   k_schur_mma<UNROLL, CTA, true, true><<<h->ntiles, CTA, 0, s>>>(h->prod.p, h->u_prod_ptr.p, h->u_row.p, h->u_col.p, h->nub, h->Z.p, h->o_lm.p,
-                                                                  h->gvec.p, h->U_val(), h->bneg(), h->tile_ptr.p, h->tile_u.p, nullptr);
+                                                                  h->gvec.p, h->U_val(), h->bneg(), h->tile_ptr.p, h->tile_u.p,
+                                                                  h->panel_on ? h->covered.p : nullptr);
 }
 
 template <int UNROLL, int CTA, bool PIPE = false>
@@ -314,7 +315,8 @@ void launch_schur(ccm_ba_handle* h, cudaStream_t s) {
     return;
   }
   if (mode == 10 && h->rs_ctas > 0) {   // off-diagonal blocks row-synchronously, diagonal blocks by the list kernel
-    k_schur_rowsync<8><<<h->rs_ctas, 32 * RS_W, 0, s>>>(h->prod.p, h->u_prod_ptr.p, h->rs_first.p, h->rs_count.p, h->Z.p, h->U_val());
+    k_schur_rowsync<8><<<h->rs_ctas, 32 * RS_W, 0, s>>>(h->prod.p, h->u_prod_ptr.p, h->rs_first.p, h->rs_count.p, h->Z.p, h->U_val(),
+                                                         h->panel_on ? h->covered.p : nullptr);
     k_schur_mma<8, 128, true><<<div_up((long long)h->nub * 32, 128), 128, 0, s>>>(h->prod.p, h->u_prod_ptr.p, h->u_row.p, h->u_col.p, h->nub, h->Z.p,
                                                                                h->o_lm.p, h->gvec.p, h->U_val(), h->bneg(), nullptr, nullptr,
                                                                                h->panel_on ? h->covered.p : nullptr, 1);
@@ -353,7 +355,8 @@ void launch_schur(ccm_ba_handle* h, cudaStream_t s) {
   switch (mode) {
     case 0:
       k_schur<<<div_up((long long)h->nub * 32, TPB), TPB, 0, s>>>(h->prod.p, h->u_prod_ptr.p, h->u_row.p, h->u_col.p, h->nub, h->Z.p,
-                                                                  h->o_lm.p, h->gvec.p, h->U_val(), h->bneg());
+                                                                  h->o_lm.p, h->gvec.p, h->U_val(), h->bneg(),
+                                                                  h->panel_on ? h->covered.p : nullptr);
       break;
     // launch shapes of the list kernel for tuning runs (tools/schur_variants.py)
     case 2: launch_schur_mma<16, 256>(h, s); break;
@@ -372,6 +375,16 @@ void step_schur(ccm_ba_handle* h) {
   KernelSpan sp(h, CCM_BA_K_SCHUR);
   launch_schur(h, h->stream);
   CCM_LAUNCHED();
+}
+
+// the CCM_SCHUR mode launch_schur actually runs: 9 without a tile schedule and 10 without a row schedule fall through to the
+// prefetching list kernel, which is mode 8
+int schur_path(const ccm_ba_handle* h) {
+  const int mode = schur_mode();
+  if (h->quad_built) return mode;
+  if (mode == 10) return h->rs_ctas > 0 ? 10 : 8;
+  if (mode == 9) return h->ntiles > 0 ? 9 : 8;
+  return mode;
 }
 
 void step_finalize(ccm_ba_handle* h, double lambda) {
@@ -1454,6 +1467,65 @@ extern "C" int ccm_ba_debug_schur(ccm_ba_handle* h, int robust, double huber_del
             for (int cc = 0; cc < 6; cc++) S_dense[(gi + rr) * n + gj + cc] = v[(size_t)q * 36 + rr * 6 + cc];
         }
     }
+  });
+}
+
+extern "C" int ccm_ba_debug_schur_blocks(ccm_ba_handle* h, int32_t* rowptr, int32_t* col, double* val, double* bschur) {
+  return guarded([&] {
+    CCM_REQUIRE(h, "null handle");
+    CCM_REQUIRE(h->nranks == 1, "debug entry points are single-rank");
+    CCM_CUDA(cudaSetDevice(h->device));
+    cudaStream_t s = h->stream;
+    const int K = h->K, Kf = h->Kf;
+    const long long nnzb = h->nnzb;
+    std::vector<int> rp((size_t)Kf + 1, 0), cl((size_t)std::max<long long>(nnzb, 1));
+    std::vector<double> v((size_t)std::max<long long>(nnzb * 36, 1)), hb((size_t)std::max(Kf * 6, 1));
+    if (Kf > 0) {
+      h->s_rowptr.download(rp.data(), rp.size(), s);
+      if (nnzb) { h->s_col.download(cl.data(), nnzb, s); h->s_val.download(v.data(), (size_t)nnzb * 36, s); }
+      h->bschur.download(hb.data(), (size_t)Kf * 6, s);
+    }
+    CCM_CUDA(cudaStreamSynchronize(s));
+    // slots are numbered in increasing pose order, so the slot-ordered rows and columns stay sorted in pose indices
+    long long q = 0;
+    for (int k = 0; k < K; k++) {
+      if (rowptr) rowptr[k] = (int32_t)q;
+      const int a = h->h_pose_slot[k];
+      if (a < 0) continue;
+      for (int t = rp[a]; t < rp[a + 1]; t++, q++) {
+        if (col) col[q] = h->h_slot_pose[cl[t]];
+        if (val) memcpy(val + (size_t)q * 36, v.data() + (size_t)t * 36, 36 * sizeof(double));
+      }
+    }
+    if (rowptr) rowptr[K] = (int32_t)q;
+    if (bschur) {
+      memset(bschur, 0, sizeof(double) * 6 * (size_t)K);
+      for (int a = 0; a < Kf; a++) memcpy(bschur + 6 * (size_t)h->h_slot_pose[a], hb.data() + (size_t)a * 6, 6 * sizeof(double));
+    }
+  });
+}
+
+extern "C" int ccm_ba_debug_paths(ccm_ba_handle* h, int32_t* out) {
+  return guarded([&] {
+    CCM_REQUIRE(h && out, "null argument");
+    CCM_CUDA(cudaSetDevice(h->device));
+    int pan = 0, cov = 0;
+    if (h->panel_on) {
+      std::vector<unsigned char> po(h->npan), cv(h->nub);
+      h->pan_on.download(po.data(), po.size(), h->stream);
+      h->covered.download(cv.data(), cv.size(), h->stream);
+      CCM_CUDA(cudaStreamSynchronize(h->stream));
+      for (unsigned char c : po) pan += c;
+      for (unsigned char c : cv) cov += c;
+    }
+    out[0] = schur_path(h);
+    out[1] = pan;
+    out[2] = h->panel_on ? h->npan : 0;
+    out[3] = cov;
+    out[4] = h->p2.on ? 2 : 1;
+    out[5] = h->pcg_block;
+    out[6] = h->pcg_agg;
+    out[7] = h->pcg_nc;
   });
 }
 

@@ -206,6 +206,65 @@ def make_local_ba(n_local=15, n_fixed=10, P=2000, obs_per_point=6, seed=1, name=
     return p
 
 
+def make_awkward_ba(seed=21) -> BAProblem:
+    """A global-BA problem built to sit on the edges of the Schur kernels' schedules (tests/test_gpu_schur.py asserts each feature):
+    199 free keyframes (not a multiple of the 8-row panel or of a 3 / 4 tile edge), fixed keyframes inside panels, co-observations
+    at free-pose offsets 43, 44 (the panel band edge) and beyond, landmarks with more than 160 observations (a panel stage cannot
+    hold them), runs of two-observation landmarks (stages capped at 32 landmarks), one keyframe pair sharing more than 4096
+    landmarks, a landmark only fixed keyframes see, one seen once, edges with flag bits 0 and 1, and observations in shuffled order.
+    The added landmarks are not geometrically consistent (only the linear system at the initial state is of interest)."""
+    rng = np.random.default_rng(seed)
+    p = make_global_ba(203, 3000, 6, window=50, n_agents=1, seed=seed)
+    K = p.K
+    fixed = np.zeros(K, np.uint8)
+    fixed[[0, 13, 50, 101]] = 1                       # 199 free; 13, 50 and 101 sit inside panels of the free poses
+    free_idx = np.flatnonzero(fixed == 0)
+    obs = [(p.obs_kf, p.obs_mp, p.obs_uv, p.obs_w)]
+    pts = [p.points]
+    centre = [np.bincount(p.obs_mp, weights=p.obs_kf, minlength=p.P) / np.maximum(np.bincount(p.obs_mp, minlength=p.P), 1)]
+    nxt = p.P
+
+    def add(kfs):
+        nonlocal nxt
+        kfs = np.asarray(kfs, np.int32)
+        n = kfs.size
+        uv = np.stack([rng.uniform(0, 752, n), rng.uniform(0, 480, n)], 1).astype(np.float32)
+        w = (1.0 / SCALE_FACTOR ** (2 * rng.integers(0, 8, n))).astype(np.float32)
+        obs.append((kfs, np.full(n, nxt, np.int32), uv, w))
+        pts.append(np.array([[rng.uniform(-0.5, 0.5), rng.uniform(-0.5, 0.5), rng.uniform(0.0, 0.4)]]).astype(np.float32).astype(np.float64))
+        centre.append(np.array([kfs.mean()]))
+        nxt += 1
+
+    a = free_idx[30]
+    for d in (43, 44, 47, 60):                        # free-pose offsets at and beyond the band edge
+        add([a, free_idx[30 + d]])
+    for _ in range(2):                                # more observations than a panel stage holds
+        add(np.sort(rng.choice(np.arange(20, 200), 170, replace=False)))
+    for _ in range(4200):                             # one pair of keyframes sharing > 4096 landmarks, as two-observation landmarks
+        add([free_idx[70], free_idx[71]])
+    add([0, 13])                                      # seen only by fixed keyframes
+    add([free_idx[120]])                              # seen once
+    kf = np.concatenate([o[0] for o in obs]); mp = np.concatenate([o[1] for o in obs])
+    uv = np.concatenate([o[2] for o in obs]); w = np.concatenate([o[3] for o in obs])
+    points = np.concatenate(pts)
+    # landmark numbering by mean observing keyframe, as a map's landmark order follows its trajectory
+    order = np.argsort(np.concatenate(centre), kind="stable")
+    relabel = np.empty_like(order); relabel[order] = np.arange(order.size)
+    mp = relabel[mp].astype(np.int32); points = points[order]
+    flags = np.zeros(kf.size, np.uint8)
+    u = rng.random(kf.size)
+    flags[u < 0.03] = 1                               # level 1: left out of the optimisation
+    flags[(u >= 0.03) & (u < 0.3)] = 2                # no robust kernel
+    perm = rng.permutation(kf.size)                   # not grouped by landmark
+    p.fixed = fixed
+    p.points = np.ascontiguousarray(points)
+    p.obs_kf, p.obs_mp = np.ascontiguousarray(kf[perm]), np.ascontiguousarray(mp[perm])
+    p.obs_uv, p.obs_w, p.edge_flags = np.ascontiguousarray(uv[perm]), np.ascontiguousarray(w[perm]), flags[perm]
+    p.gt_points = None
+    p.name = "awkward"
+    return p
+
+
 def make_config(name: str, **over) -> BAProblem:
     cfg = dict(CONFIGS[name]); cfg.update(over)
     kind = cfg.pop("kind")

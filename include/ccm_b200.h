@@ -167,6 +167,15 @@ int ccm_ba_debug_build(ccm_ba_handle* h, int robust, double huber_delta,
 int ccm_ba_debug_schur(ccm_ba_handle* h, int robust, double huber_delta, double lambda,
                        double* S_dense /*(6K)^2 or NULL*/, double* bschur /*6K or NULL*/,
                        double* dx_pose /*K*6*/, double* dx_point /*P*3*/, int32_t* pcg_iters, double* pcg_relres);
+/* S (lambda included) and b_schur as the last ccm_ba_debug_schur left them, as block CSR in the caller's pose indices: every stored
+ * 6x6 block of the full symmetric pattern, row-major, columns ascending; fixed poses have empty rows and zero b_schur.
+ * nnzb = ccm_ba_info.s_blocks_full.  Any output may be NULL. */
+int ccm_ba_debug_schur_blocks(ccm_ba_handle* h, int32_t* rowptr /*K+1*/, int32_t* col /*nnzb*/, double* val /*nnzb*36*/,
+                              double* bschur /*6K*/);
+/* the paths the handle runs: out[0] Schur mode in effect (CCM_SCHUR numbering; 9 / 10 without their schedule run as 8),
+ * out[1] panels enabled, out[2] panels in total (0 without CCM_SCHUR_PANEL), out[3] upper blocks the panels own,
+ * out[4] PCG implementation (1 k_pcg, 2 k_pcg2), out[5] k_pcg CTA size, out[6] coarse aggregate size, out[7] coarse nodes (0: no coarse space) */
+int ccm_ba_debug_paths(ccm_ba_handle* h, int32_t* out /*8*/);
 /* developer hook: pick the Schur-product kernel for every handle of this process: 0 = gather form (k_schur), 1 = tensor-core
  * form (k_schur_mma, one f64 mma.sync per product; the default), 2..8 = variants of it (unroll 16 / 4, CTA 64 / 256 / 512, entry prefetch; the default is unroll 8, CTA 128),
  * -1 = back to the CCM_SCHUR environment variable / built-in default */

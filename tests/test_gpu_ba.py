@@ -42,21 +42,6 @@ def test_linearisation_blocks_match_oracle(oracle, name):
     h.close()
 
 
-@pytest.mark.parametrize("name", ["tiny", "small"])
-def test_schur_system_and_step_match_oracle(oracle, name):
-    p = synth.make_config(name)
-    lam = 1e-5 * max(np.abs(np.einsum("kii->ki", oracle.ba_build(p, huber_delta=api.HUBER_GBA)["Hpp"])).max(), 1.0)
-    ref = oracle.ba_schur_solve(p, lam, huber_delta=api.HUBER_GBA, dense=True)
-    h = api.BAHandle(p)
-    got = h.debug_schur(lam, huber_delta=api.HUBER_GBA, dense=True)
-    assert _relerr(got["S"], ref["S"]) < 1e-9
-    assert _relerr(got["bschur"], ref["bschur"]) < 1e-9
-    assert got["pcg_relres"] < 1e-12
-    assert _relerr(got["dx_pose"], ref["dx_pose"]) < 1e-6
-    assert _relerr(got["dx_point"], ref["dx_point"]) < 1e-6
-    h.close()
-
-
 @pytest.mark.parametrize("name,iters", [("tiny", 12), ("small", 10), ("cfg2", 15), ("cfg3", 20)])
 def test_lm_matches_oracle_after_same_iteration_count(oracle, name, iters):
     p = synth.make_config(name)
