@@ -428,6 +428,23 @@ def gba_map_update(sc):
     return _map_update_result(a, K, P)
 
 
+def normal_depth(sc, host=False):
+    """MapPoint::UpdateNormalAndDepth (cslam/src/MapPoint.cpp:779-823) for a batch of points, see include/ccm_b200.h.  sc: dict(kf_centre
+    (K,3) f32, kf_bad (K,) u8, mp_pos (P,3) f32, obs_ptr (P+1,) i64, obs_kf (E,) i32, mp_ref (P,) i32, mp_scale_ref, mp_scale_last (P,) f32).
+    Returns dict(normal (P,3), max_dist, min_dist, status).  host=False: ccm_normal_depth on the GPU; host=True: ccm_normal_depth_host."""
+    K = len(sc["kf_bad"]); P = len(sc["mp_ref"])
+    a = dict(c=np.ascontiguousarray(sc["kf_centre"], np.float32).reshape(K, 3), bad=np.ascontiguousarray(sc["kf_bad"], np.uint8),
+             pos=np.ascontiguousarray(sc["mp_pos"], np.float32).reshape(P, 3), ptr=np.ascontiguousarray(sc["obs_ptr"], np.int64),
+             obs=np.ascontiguousarray(sc["obs_kf"], np.int32), ref=np.ascontiguousarray(sc["mp_ref"], np.int32),
+             sr=np.ascontiguousarray(sc["mp_scale_ref"], np.float32), sl=np.ascontiguousarray(sc["mp_scale_last"], np.float32))
+    out = dict(normal=np.zeros((P, 3), np.float32), max_dist=np.zeros(P, np.float32), min_dist=np.zeros(P, np.float32),
+               status=np.zeros(P, np.uint8))
+    fn = lib().ccm_normal_depth_host if host else lib().ccm_normal_depth
+    _chk(fn(K, _p(a["c"]), _p(a["bad"]), P, _p(a["pos"]), _p(a["ptr"]), _p(a["obs"]), _p(a["ref"]), _p(a["sr"]), _p(a["sl"]),
+            _p(out["normal"]), _p(out["max_dist"]), _p(out["min_dist"]), _p(out["status"])))
+    return out
+
+
 class MapMirror:
     """Persistent flat mirror of the map for the global BA (ccm_mirror_*, include/ccm_b200.h; SURVEY.md §8(f) rank 1): told about
     changes as they happen, hands out the ccm_ba_problem MapFusionGBA's flattening (S/Optimizer.cpp:658-787) would build."""

@@ -418,3 +418,74 @@ def make_map_update(K=200, P=5000, seed=0, new_kf_frac=0.15, outside_frac=0.03, 
     pos_gba[state != 1] = np.float32(np.nan)
     return dict(kf_parent=parent, kf_optimized=optimized.astype(np.uint8), kf_Tcw=Tcw, kf_TcwGBA=gba, mp_state=state, mp_ref=ref, mp_pos=pos,
                 mp_pos_gba=pos_gba)
+
+
+def scale_factors(n_levels=8, scale_factor=SCALE_FACTOR):
+    """ORBextractor's mvScaleFactor (S/ORBextractor.cpp:584-590): f32, each level the previous one times the factor"""
+    s = np.ones(n_levels, np.float32)
+    for i in range(1, n_levels):
+        s[i] = np.float32(s[i - 1] * np.float32(scale_factor))
+    return s
+
+
+def make_normal_depth(p: BAProblem | None = None, seed=0, K=60, P=2000, bad_kf_frac=0.05, bad_mp_frac=0.02, off_ref_frac=0.03,
+                      all_bad_frac=0.0, on_centre_frac=0.0, map_order=False):
+    """Inputs of ccm_normal_depth (MapPoint::UpdateNormalAndDepth over a batch, include/ccm_b200.h) for the map of a BA problem `p`
+    (None: a random one of K keyframes and P points): keyframe centres -R^T t and bad flags, every point's observers in the problem's
+    observation order, a reference keyframe among them (off_ref_frac: one that does not observe the point, whose keypoint 0 then
+    gives the octave), scale factors of an 8-level pyramid.  Bad points (bad_mp_frac) are passed with no observers, as the shim passes
+    them.  all_bad_frac: points whose observers are all bad keyframes (NaN normal); on_centre_frac: points moved onto an observer's centre.
+    map_order: each point's observers unique and in ascending row, the order a std::map<kfptr> keeps when the keyframes lie in
+    memory in row order (the stand-in scenes of the shim tests).
+    Extra keys describe the scene behind the flat arrays: obs_octave, kf_oct0, mp_bad, ref_observes."""
+    rng = np.random.default_rng(seed)
+    if p is None:
+        cen = rng.normal(0, 3.0, (K, 3)).astype(np.float32)
+        deg = rng.integers(1, 9, P)
+        obs_mp = np.repeat(np.arange(P, dtype=np.int32), deg)
+        obs_kf = rng.integers(0, K, len(obs_mp)).astype(np.int32)
+        pos = rng.normal(0, 8.0, (P, 3)).astype(np.float32)
+    else:
+        K, P = p.K, p.P
+        q = p.poses[:, :4]; t = p.poses[:, 4:7]
+        x, y, z, w = q[:, 0], q[:, 1], q[:, 2], q[:, 3]
+        R = np.stack([1 - 2 * (y * y + z * z), 2 * (x * y - z * w), 2 * (x * z + y * w),
+                      2 * (x * y + z * w), 1 - 2 * (x * x + z * z), 2 * (y * z - x * w),
+                      2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)], 1).reshape(K, 3, 3)
+        cen = (-np.einsum("kji,kj->ki", R, t)).astype(np.float32)
+        order = np.argsort(p.obs_mp, kind="stable")
+        obs_mp, obs_kf = p.obs_mp[order].astype(np.int32), p.obs_kf[order].astype(np.int32).copy()
+        pos = p.points.astype(np.float32)
+    if map_order:
+        pair = np.unique(obs_mp.astype(np.int64) * K + obs_kf)
+        obs_mp, obs_kf = (pair // K).astype(np.int32), (pair % K).astype(np.int32)
+    deg = np.bincount(obs_mp, minlength=P)
+    ptr = np.zeros(P + 1, np.int64); ptr[1:] = np.cumsum(deg)
+    kf_bad = (rng.random(K) < bad_kf_frac).astype(np.uint8)
+    mp_bad = rng.random(P) < bad_mp_frac
+    obs_octave = rng.choice(8, len(obs_kf), p=OCTAVE_QUOTAS / OCTAVE_QUOTAS.sum()).astype(np.int32)
+    kf_oct0 = rng.integers(0, 8, K).astype(np.int32)
+    bad_rows = np.flatnonzero(kf_bad)
+    if len(bad_rows):
+        for i in np.flatnonzero((rng.random(P) < all_bad_frac) & (deg > 0) & (deg <= len(bad_rows))):
+            pick = rng.choice(bad_rows, deg[i], replace=False)
+            obs_kf[ptr[i]:ptr[i + 1]] = np.sort(pick) if map_order else pick
+    sf = scale_factors()
+    ref = np.full(P, -1, np.int32); ref_observes = np.zeros(P, bool); sref = np.ones(P, np.float32)
+    for i in np.flatnonzero(deg > 0):
+        b, e = ptr[i], ptr[i + 1]
+        if rng.random() < off_ref_frac:
+            ref[i] = rng.integers(0, K)
+        else:
+            ref[i] = obs_kf[rng.integers(b, e)]
+        hit = np.flatnonzero(obs_kf[b:e] == ref[i])
+        ref_observes[i] = len(hit) > 0
+        sref[i] = sf[obs_octave[b + hit[0]]] if len(hit) else sf[kf_oct0[ref[i]]]
+    for i in np.flatnonzero((rng.random(P) < on_centre_frac) & (deg > 0)):
+        pos[i] = cen[obs_kf[ptr[i]]]
+    keep = np.repeat(~mp_bad, deg)                              # a bad point goes in with no observers
+    dk = np.where(mp_bad, 0, deg)
+    fptr = np.zeros(P + 1, np.int64); fptr[1:] = np.cumsum(dk)
+    return dict(kf_centre=cen, kf_bad=kf_bad, mp_pos=pos, obs_ptr=fptr, obs_kf=obs_kf[keep], mp_ref=ref, mp_scale_ref=sref,
+                mp_scale_last=np.full(P, sf[-1], np.float32), obs_octave=obs_octave[keep], kf_oct0=kf_oct0, mp_bad=mp_bad,
+                ref_observes=ref_observes)

@@ -604,6 +604,29 @@ int ccm_kfdb_get_timing(ccm_kfdb* h, double* count_ms, double* score_ms, int64_t
 int ccm_kfdb_select(const ccm_kfdb_result* r, const int32_t* covis_ptr, const uint64_t* covis_uid, int32_t reloc, float min_score,
                     uint64_t* out_uid, int32_t* n_out);
 
+/* ---- map-point normals and depth limits ------------------------------------------------------------------------------
+ * MapPoint::UpdateNormalAndDepth (cslam/src/MapPoint.cpp:779-823) for a batch of points, bit for bit (f32 as OpenCV evaluates each
+ * cv::Mat expression; see ccm_slam_b200/csrc/normal_depth_math.cuh).
+ *   kf_centre [n_kf][3]   GetCameraCenter() of each keyframe row;  kf_bad [n_kf]: isBad() (a bad observer is skipped and not counted)
+ *   mp_pos [n_mp][3]      mWorldPos
+ *   obs_ptr [n_mp+1], obs_kf [obs_ptr[n_mp]]   the observers of point i, obs_kf[obs_ptr[i] .. obs_ptr[i+1]), in mObservations order
+ *                         (the normal is an f32 sum over them: the order is kept as given)
+ *   mp_ref [n_mp]         row of mpRefKF (used even when bad); -1: none
+ *   mp_scale_ref          pRefKF->mvScaleFactors[octave of mvKeysUn[observations[pRefKF]]] (index 0 when pRefKF does not observe it:
+ *                         the reference's operator[] inserts 0)
+ *   mp_scale_last         pRefKF->mvScaleFactors[mnScaleLevels - 1]
+ * Out: normal [n_mp][3] (mNormalVector), max_dist (mfMaxDistance), min_dist (mfMinDistance), status [n_mp]: 1 written, 0 untouched
+ * (no observers, or mp_ref = -1; a bad point is passed with no observers).  Untouched points read 0 in every output.  Every observer
+ * bad gives NaN in the normal, a point on an observer's centre too: both are the reference's values.
+ * ccm_normal_depth runs on the GPU (host buffers in and out, its own stream); ccm_normal_depth_host is the same contract on the host,
+ * usable without a device, for the single points tracking and mapping update one at a time. */
+int ccm_normal_depth(int32_t n_kf, const float* kf_centre, const uint8_t* kf_bad, int32_t n_mp, const float* mp_pos, const int64_t* obs_ptr,
+                     const int32_t* obs_kf, const int32_t* mp_ref, const float* mp_scale_ref, const float* mp_scale_last, float* normal,
+                     float* max_dist, float* min_dist, uint8_t* status);
+int ccm_normal_depth_host(int32_t n_kf, const float* kf_centre, const uint8_t* kf_bad, int32_t n_mp, const float* mp_pos, const int64_t* obs_ptr,
+                          const int32_t* obs_kf, const int32_t* mp_ref, const float* mp_scale_ref, const float* mp_scale_last, float* normal,
+                          float* max_dist, float* min_dist, uint8_t* status);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1,0 +1,2 @@
+// see Frame.h in this directory
+#include <cslam/Frame.h>

@@ -14,9 +14,15 @@
 #include <mutex>
 #include <unordered_map>
 
+#include "MapPoint_shim.h"
 #include "ccm_b200.h"
 
 namespace cslam {
+
+// shim/MapPoint_shim.cpp defines these.  A build that keeps the reference's own MapPoint.cpp links the no-ops below instead: the
+// write-back loops then leave every UpdateNormalAndDepth() to the reference body, point by point.
+__attribute__((weak)) void ccm_b200_prepare_normals(const vector<boost::shared_ptr<MapPoint> >&, const float*) {}
+__attribute__((weak)) void ccm_b200_clear_normals() {}
 
 namespace {
 
@@ -71,6 +77,13 @@ cv::Mat point_to_cv(const double* x) {
   for (int i = 0; i < 3; i++) X.at<float>(i) = (float)x[i];
   return X;
 }
+// the points a write-back loop is about to SetWorldPos + UpdateNormalAndDepth, with the f32 positions they will take
+struct NormalBatch {
+  vector<boost::shared_ptr<MapPoint> > mps;
+  vector<float> pos;
+  void add(const boost::shared_ptr<MapPoint>& pMP, const double* x) { mps.push_back(pMP); for (int i = 0; i < 3; i++) pos.push_back((float)x[i]); }
+  void prepare() const { ccm_b200_prepare_normals(mps, pos.data()); }
+};
 void check(int rc) { if (rc != CCM_OK) { std::cerr << "libccm_b200: " << ccm_last_error() << std::endl; throw estd::infrastructure_ex(); } }
 
 // Optional persistent mirrors (INTEGRATION.md 4a, SURVEY.md 8(f) rank 1): a server that keeps a ccm_map_mirror up to date for a Map
@@ -154,6 +167,15 @@ void Optimizer::MapFusionGBA(mapptr pMap, size_t ClientId, int nIterations, bool
       if (nLoopKF == zeropair) it->second->SetPose(T, true);
       else { it->second->mTcwGBA.create(4, 4, CV_32F); T.copyTo(it->second->mTcwGBA); it->second->mBAGlobalForKF = nLoopKF; }
     }
+    ParkedNormalsGuard parked_normals;
+    if (nLoopKF == zeropair) {                                // every UpdateNormalAndDepth() below in one device call
+      NormalBatch nb;
+      for (int r = 0; r < prob.P; r++) {
+        auto it = mp_of_uid.find(mp_uid[r]);
+        if (it != mp_of_uid.end() && !it->second->isBad()) nb.add(it->second, &points[3 * (size_t)r]);
+      }
+      nb.prepare();
+    }
     for (int r = 0; r < prob.P; r++) {                        // :827-857
       auto it = mp_of_uid.find(mp_uid[r]);
       if (it == mp_of_uid.end() || it->second->isBad()) continue;
@@ -213,6 +235,13 @@ void Optimizer::MapFusionGBA(mapptr pMap, size_t ClientId, int nIterations, bool
     if (nLoopKF == zeropair) pKF->SetPose(T, true);
     else { pKF->mTcwGBA.create(4, 4, CV_32F); T.copyTo(pKF->mTcwGBA); pKF->mBAGlobalForKF = nLoopKF; }
   }
+  ParkedNormalsGuard parked_normals;
+  if (nLoopKF == zeropair) {
+    NormalBatch nb;
+    for (size_t i = 0; i < vpMP.size(); i++)
+      if (mp_row[i] >= 0 && !vpMP[i]->isBad()) nb.add(vpMP[i], &points[3 * (size_t)mp_row[i]]);
+    nb.prepare();
+  }
   for (size_t i = 0; i < vpMP.size(); i++) {                  // :827-857
     if (mp_row[i] < 0) continue;
     mpptr pMP = vpMP[i];
@@ -268,6 +297,13 @@ void Optimizer::BundleAdjustmentClient(const vector<kfptr>& vpKFs, const vector<
     cv::Mat T = pose_to_cv(&poses[7 * (size_t)kf_row[i]]);
     if (nLoopKF == zeropair) pKF->SetPose(T, false);
     else { pKF->mTcwGBA.create(4, 4, CV_32F); T.copyTo(pKF->mTcwGBA); pKF->mBAGlobalForKF = nLoopKF; }
+  }
+  ParkedNormalsGuard parked_normals;
+  if (nLoopKF == zeropair) {
+    NormalBatch nb;
+    for (size_t i = 0; i < vpMP.size(); i++)
+      if (mp_row[i] >= 0 && !vpMP[i]->isBad()) nb.add(vpMP[i], &points[3 * (size_t)mp_row[i]]);
+    nb.prepare();
   }
   for (size_t i = 0; i < vpMP.size(); i++) {
     if (mp_row[i] < 0 || vpMP[i]->isBad()) continue;
@@ -350,6 +386,13 @@ void Optimizer::LocalBundleAdjustmentClient(kfptr pKF, bool* pbStopFlag, mapptr 
   for (auto& e : vToErase) { e.first->EraseMapPointMatch(e.second); e.second->EraseObservation(e.first); }
   size_t row = 0;
   for (kfptr k : lLocalKeyFrames) { k->SetPose(pose_to_cv(&poses[7 * row++]), false); k->mbUpdatedByServer = false; }
+  ParkedNormalsGuard parked_normals;
+  {
+    NormalBatch nb;
+    for (size_t i = 0; i < mp_rows.size(); i++)
+      if (!mp_rows[i]->isBad()) nb.add(mp_rows[i], &points[3 * i]);
+    nb.prepare();
+  }
   for (size_t i = 0; i < mp_rows.size(); i++) {
     mpptr pMP = mp_rows[i];
     if (pMP->isBad()) { if (pMap->GetMpPtr(pMP->mId)) throw estd::infrastructure_ex(); continue; }
@@ -485,6 +528,10 @@ void optimize_essential_graph(Optimizer::mapptr pMap, Optimizer::kfptr pLoopKF, 
     tv *= (1. / s);
     kfi->SetPose(Converter::toCvSE3(Rm, tv), true);
   }
+  // every x_new first, then one device call for the normals, then the write-back in the same order as before
+  vector<size_t> moved;
+  vector<Eigen::Matrix<double, 3, 1> > x_news;
+  NormalBatch nb;
   for (size_t i = 0; i < mps.size(); i++) {
     mpptr mp = mps[i];
     if (mp->isBad()) continue;
@@ -495,7 +542,15 @@ void optimize_essential_graph(Optimizer::mapptr pMap, Optimizer::kfptr pLoopKF, 
     if (!S_cw.count(id_ref)) continue;                           // reference keyframe not in the graph
     Eigen::Matrix<double, 3, 1> x_old = Converter::toVector3d(mp->GetWorldPos());
     Eigen::Matrix<double, 3, 1> x_new = S_wc_new.find(id_ref)->second.map(S_cw.find(id_ref)->second.map(x_old));
-    mp->SetWorldPos(Converter::toCvMat(x_new), true);
+    moved.push_back(i); x_news.push_back(x_new);
+    const double x[3] = {x_new[0], x_new[1], x_new[2]};
+    nb.add(mp, x);                                               // Converter::toCvMat(x_new): each component rounded to float
+  }
+  ParkedNormalsGuard parked_normals;
+  nb.prepare();
+  for (size_t j = 0; j < moved.size(); j++) {
+    mpptr mp = mps[moved[j]];
+    mp->SetWorldPos(Converter::toCvMat(x_news[j]), true);
     mp->UpdateNormalAndDepth();
   }
 }
