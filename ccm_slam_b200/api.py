@@ -445,6 +445,20 @@ def normal_depth(sc, host=False):
     return out
 
 
+
+def distinctive_descriptors(sc, host=False):
+    """MapPoint::ComputeDistinctiveDescriptors (cslam/src/MapPoint.cpp:929-994) for a batch of points, see include/ccm_b200.h.  sc: dict(
+    kf_bad (K,) u8, obs_ptr (P+1,) i64, obs_kf (E,) i32, obs_desc (E,32) u8), as synth.make_distinctive builds it.  Returns dict(best (P,)
+    i32: position of the chosen observer in the point's list, -1 untouched; best_median (P,) i32; desc (P,32) u8).  host=False:
+    ccm_distinctive_descriptors on the GPU; host=True: ccm_distinctive_descriptors_host."""
+    K = len(sc["kf_bad"]); P = len(sc["obs_ptr"]) - 1
+    a = dict(bad=np.ascontiguousarray(sc["kf_bad"], np.uint8), ptr=np.ascontiguousarray(sc["obs_ptr"], np.int64),
+             obs=np.ascontiguousarray(sc["obs_kf"], np.int32), desc=np.ascontiguousarray(sc["obs_desc"], np.uint8).reshape(-1, 32))
+    out = dict(best=np.zeros(P, np.int32), best_median=np.zeros(P, np.int32), desc=np.zeros((P, 32), np.uint8))
+    fn = lib().ccm_distinctive_descriptors_host if host else lib().ccm_distinctive_descriptors
+    _chk(fn(K, _p(a["bad"]), P, _p(a["ptr"]), _p(a["obs"]), _p(a["desc"]), _p(out["best"]), _p(out["best_median"]), _p(out["desc"])))
+    return out
+
 class MapMirror:
     """Persistent flat mirror of the map for the global BA (ccm_mirror_*, include/ccm_b200.h; SURVEY.md §8(f) rank 1): told about
     changes as they happen, hands out the ccm_ba_problem MapFusionGBA's flattening (S/Optimizer.cpp:658-787) would build."""

@@ -66,6 +66,23 @@ struct ccm_kf_store {
   }
 };
 
+namespace ccm {
+// the device address of each uid's first descriptor and its feature count (nullptr / -1: not in the store), for
+// ccm_kfstore_distinctive_descriptors (distinctive.cu); read under the store's lock, like every matcher's operands
+void kfstore_resolve(ccm_kf_store* s, int32_t n, const uint64_t* uid, std::vector<const uint4*>& base, std::vector<int32_t>& n_feat,
+                     int* device) {
+  std::lock_guard<std::mutex> lock(s->mu);
+  base.assign(n, nullptr); n_feat.assign(n, -1);
+  for (int32_t k = 0; k < n; k++) {
+    auto it = s->kf.find(uid[k]);
+    if (it == s->kf.end()) continue;
+    n_feat[k] = (int32_t)it->second.r.n;
+    base[k] = it->second.r.n ? s->ptr(it->second.r) : nullptr;
+  }
+  *device = s->device;
+}
+}  // namespace ccm
+
 namespace {
 // ccmslam_msgs/CvKeyPoint as ROS serialises it: f32 x, f32 y, u8 size, f32 angle, u8 response, i8 octave (15 bytes, packed)
 constexpr int WIRE_KP = 15;

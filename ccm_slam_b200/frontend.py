@@ -414,6 +414,18 @@ class KeyFrameStore:
         return dict(word=word, node=node, weight=weight, bow_id=bow_id[:bn.value].copy(), bow_val=bow_val[:bn.value].copy(),
                     fv_node_id=fid[:fn.value].copy(), fv_node_ptr=fptr[:fn.value + 1].copy(), fv_feat=ffeat[:fptr[fn.value] if fn.value else 0].copy())
 
+    def distinctive_descriptors(self, kf_uid, kf_bad, obs_ptr, obs_kf, obs_feat):
+        """MapPoint::ComputeDistinctiveDescriptors for a batch of points over the resident descriptors (ccm_kfstore_distinctive_descriptors):
+        keyframe row k is uid kf_uid[k]; observation j is feature obs_feat[j] of row obs_kf[j].  Returns dict(best, best_median, desc)
+        as api.distinctive_descriptors."""
+        uid = np.ascontiguousarray(kf_uid, np.uint64); bad = np.ascontiguousarray(kf_bad, np.uint8)
+        ptr = np.ascontiguousarray(obs_ptr, np.int64); okf = np.ascontiguousarray(obs_kf, np.int32); feat = np.ascontiguousarray(obs_feat, np.int32)
+        P = len(ptr) - 1
+        out = dict(best=np.zeros(P, np.int32), best_median=np.zeros(P, np.int32), desc=np.zeros((P, 32), np.uint8))
+        _chk(lib().ccm_kfstore_distinctive_descriptors(self._h, len(uid), _p(uid), _p(bad), P, _p(ptr), _p(okf), _p(feat), _p(out["best"]),
+                                                       _p(out["best_median"]), _p(out["desc"])))
+        return out
+
     def __del__(self):
         try:
             self.close()

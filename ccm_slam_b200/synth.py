@@ -489,3 +489,80 @@ def make_normal_depth(p: BAProblem | None = None, seed=0, K=60, P=2000, bad_kf_f
     return dict(kf_centre=cen, kf_bad=kf_bad, mp_pos=pos, obs_ptr=fptr, obs_kf=obs_kf[keep], mp_ref=ref, mp_scale_ref=sref,
                 mp_scale_last=np.full(P, sf[-1], np.float32), obs_octave=obs_octave[keep], kf_oct0=kf_oct0, mp_bad=mp_bad,
                 ref_observes=ref_observes)
+
+
+def make_distinctive(p: BAProblem | None = None, seed=0, K=60, P=2000, max_deg=8, bad_kf_frac=0.05, bad_mp_frac=0.0, all_bad_frac=0.0,
+                     empty_frac=0.0, forced_n=(), extra_feat=8, map_order=False):
+    """Inputs of ccm_distinctive_descriptors (MapPoint::ComputeDistinctiveDescriptors over a batch, include/ccm_b200.h) for the
+    observation lists of a BA problem `p` (None: a random map of K keyframes and P points, 1..max_deg observers each).
+    Every point has a "true" 32-byte descriptor; each observation of it is that descriptor with random bit flips at a per-point rate
+    (none, 1/128 .. 1/8), so rows repeat and medians tie often.  Each keyframe holds its observed features, at shuffled indices, plus
+    up to extra_feat unobserved ones.  bad_kf_frac: bad keyframes (skipped observers); all_bad_frac: points whose observers are all
+    bad; empty_frac: points with no observers; bad_mp_frac: bad points, passed with no observers as the shim passes them; forced_n:
+    extra points appended at the end, one per value, with exactly that many observers, all of keyframes that are not bad.
+    map_order: each point's observers unique and in ascending row (the order std::map<kfptr> keeps for the stand-in scenes).
+    Returns kf_bad, kf_uid (u64), kf_nfeat, kf_desc_ptr (K+1), kf_desc (sum nfeat, 32), obs_ptr, obs_kf, obs_feat, obs_desc (E, 32),
+    mp_bad."""
+    rng = np.random.default_rng(seed)
+    if p is None:
+        deg = rng.integers(1, max_deg + 1, P)
+        obs_mp = np.repeat(np.arange(P, dtype=np.int64), deg)
+        obs_kf = rng.integers(0, K, len(obs_mp)).astype(np.int64)
+    else:
+        K, P = p.K, p.P
+        order = np.argsort(p.obs_mp, kind="stable")
+        obs_mp, obs_kf = p.obs_mp[order].astype(np.int64), p.obs_kf[order].astype(np.int64)
+    if map_order:
+        pair = np.unique(obs_mp * K + obs_kf)
+        obs_mp, obs_kf = pair // K, pair % K
+    kf_bad = (rng.random(K) < bad_kf_frac).astype(np.uint8)
+    good = np.flatnonzero(kf_bad == 0)
+    if len(forced_n):
+        add_mp, add_kf = [], []
+        for t, n in enumerate(forced_n):
+            pick = rng.choice(good, n, replace=n > len(good) and not map_order)
+            add_mp.append(np.full(n, P + t, np.int64)); add_kf.append(np.sort(pick) if map_order else pick)
+        obs_mp = np.concatenate([obs_mp] + add_mp); obs_kf = np.concatenate([obs_kf] + add_kf)
+        P += len(forced_n)
+    n_forced = len(forced_n)
+    free = np.arange(P) < P - n_forced
+    empty = free & (rng.random(P) < empty_frac)
+    obs_keep = ~empty[obs_mp]
+    obs_mp, obs_kf = obs_mp[obs_keep], obs_kf[obs_keep]
+    deg = np.bincount(obs_mp, minlength=P)
+    ptr = np.zeros(P + 1, np.int64); ptr[1:] = np.cumsum(deg)
+    bad_rows = np.flatnonzero(kf_bad)
+    if len(bad_rows):
+        for i in np.flatnonzero(free & (rng.random(P) < all_bad_frac) & (deg > 0) & (deg <= len(bad_rows))):
+            pick = rng.choice(bad_rows, deg[i], replace=False)
+            obs_kf[ptr[i]:ptr[i + 1]] = np.sort(pick) if map_order else pick
+    mp_bad = free & (rng.random(P) < bad_mp_frac)
+    keep = np.repeat(~mp_bad, deg)                              # a bad point goes in with no observers
+    obs_mp, obs_kf = obs_mp[keep], obs_kf[keep]
+    deg = np.where(mp_bad, 0, deg)
+    ptr = np.zeros(P + 1, np.int64); ptr[1:] = np.cumsum(deg)
+    E = len(obs_kf)
+    # descriptors: truth xor a mask whose bits are set with probability 2^-m (m per point; m = 0: an exact copy)
+    truth = rng.integers(0, 256, (P, 32), dtype=np.uint8)
+    m_pt = rng.choice(np.array([0, 3, 4, 5, 6, 7]), P)
+    obs_desc = np.empty((E, 32), np.uint8)
+    for c0 in range(0, E, 1 << 20):
+        c1 = min(E, c0 + (1 << 20))
+        m = m_pt[obs_mp[c0:c1]][:, None]
+        mask = np.where(m > 0, np.uint8(255), np.uint8(0)) * np.ones((1, 32), np.uint8)
+        for r in range(7):
+            mask &= np.where(r < m, rng.integers(0, 256, (c1 - c0, 32), dtype=np.uint8), np.uint8(255))
+        obs_desc[c0:c1] = truth[obs_mp[c0:c1]] ^ mask
+    # features: each keyframe's observations at shuffled indices, then unobserved features
+    order = np.lexsort((rng.random(E), obs_kf))
+    per_kf = np.bincount(obs_kf, minlength=K)
+    start = np.zeros(K + 1, np.int64); start[1:] = np.cumsum(per_kf)
+    obs_feat = np.empty(E, np.int64)
+    obs_feat[order] = np.arange(E) - start[obs_kf[order]]
+    nfeat = per_kf + rng.integers(0, extra_feat + 1, K)
+    kptr = np.zeros(K + 1, np.int64); kptr[1:] = np.cumsum(nfeat)
+    kf_desc = rng.integers(0, 256, (int(kptr[-1]), 32), dtype=np.uint8)
+    kf_desc[kptr[obs_kf] + obs_feat] = obs_desc
+    kf_uid = (np.uint64(3) << np.uint64(40)) + np.arange(K, dtype=np.uint64) * np.uint64(7) + np.uint64(11)
+    return dict(kf_bad=kf_bad, kf_uid=kf_uid, kf_nfeat=nfeat.astype(np.int32), kf_desc_ptr=kptr, kf_desc=kf_desc, obs_ptr=ptr,
+                obs_kf=obs_kf.astype(np.int32), obs_feat=obs_feat.astype(np.int32), obs_desc=obs_desc, mp_bad=mp_bad)

@@ -627,6 +627,31 @@ int ccm_normal_depth_host(int32_t n_kf, const float* kf_centre, const uint8_t* k
                           const int32_t* obs_kf, const int32_t* mp_ref, const float* mp_scale_ref, const float* mp_scale_last, float* normal,
                           float* max_dist, float* min_dist, uint8_t* status);
 
+/* ---- map-point descriptors ------------------------------------------------------------------------------------------
+ * MapPoint::ComputeDistinctiveDescriptors (cslam/src/MapPoint.cpp:929-994) for a batch of points, exactly (integer work): among the
+ * observers that are not bad, the row whose median Hamming distance to all of them (itself included, the ((N-1)/2)-th smallest: the
+ * lower middle for even N) is the first strictly smallest.  Any N; the reference's stack array limits it to about 1400.
+ *   kf_bad [n_kf]         isBad() of each keyframe row (a bad observer is skipped: neither a candidate nor counted in N)
+ *   obs_ptr [n_mp+1], obs_kf [obs_ptr[n_mp]]   the observers of point i, obs_kf[obs_ptr[i] .. obs_ptr[i+1]), in mObservations order
+ *   obs_desc [E][32]      pKF->mDescriptors.row(idx) of each observation (read only for observers that are not bad)
+ * Out: best [n_mp]        position of the chosen observer IN THE CALLER'S LIST obs_ptr[i] .. obs_ptr[i+1), bad observers counted, so
+ *                         that it maps straight back to (pKF, idx); -1: untouched (no observers, or every observer bad; a bad point
+ *                         is passed with no observers)
+ *      best_median [n_mp] the chosen row's median (or NULL); desc_out [n_mp][32] its bytes (or NULL).  Untouched points read 0.
+ * ccm_distinctive_descriptors runs on the GPU (host buffers in and out, its own stream); ccm_distinctive_descriptors_host is the same
+ * contract on the host, usable without a device, for the single points that mapping and map merging update one at a time.
+ * ccm_kfstore_distinctive_descriptors reads the rows from the keyframe store instead: kf_uid [n_kf] names each row's keyframe
+ * (mUniqueId), obs_feat [E] the feature index (idx), so 8 bytes per observation cross the bus and ccm_kfstore_h2d_bytes does not
+ * move.  An unknown uid or a feature index outside [0, N of the keyframe) of an observer that is not bad, or any keyframe row out of
+ * range, fails the call with CCM_ERR_INVALID and a message naming the point; no output is written then. */
+int ccm_distinctive_descriptors(int32_t n_kf, const uint8_t* kf_bad, int32_t n_mp, const int64_t* obs_ptr, const int32_t* obs_kf,
+                                const uint8_t* obs_desc, int32_t* best, int32_t* best_median, uint8_t* desc_out);
+int ccm_distinctive_descriptors_host(int32_t n_kf, const uint8_t* kf_bad, int32_t n_mp, const int64_t* obs_ptr, const int32_t* obs_kf,
+                                     const uint8_t* obs_desc, int32_t* best, int32_t* best_median, uint8_t* desc_out);
+int ccm_kfstore_distinctive_descriptors(ccm_kf_store* store, int32_t n_kf, const uint64_t* kf_uid, const uint8_t* kf_bad, int32_t n_mp,
+                                        const int64_t* obs_ptr, const int32_t* obs_kf, const int32_t* obs_feat, int32_t* best,
+                                        int32_t* best_median, uint8_t* desc_out);
+
 #ifdef __cplusplus
 }
 #endif
