@@ -336,6 +336,56 @@ def pgo_solve(p, iterations=20, lambda_init=1e-16, pcg_max_iter=0, pcg_tol=0.0, 
                 chi2_final=res.chi2_final, lambda_final=res.lambda_final, t_total_ms=res.t_total_ms)
 
 
+def sim3_debug_ops(u, a, b, fix_scale=False):
+    """ccm_sim3_debug_ops: the device's s3_exp(u), s3_log(a), s3_mul(a, b), s3_inv(a), s3_oplus(a, u) row by row"""
+    u = np.ascontiguousarray(u, np.float64).reshape(-1, 7); a = np.ascontiguousarray(a, np.float64).reshape(-1, 8)
+    b = np.ascontiguousarray(b, np.float64).reshape(-1, 8)
+    n = u.shape[0]
+    assert a.shape[0] == n and b.shape[0] == n
+    out = dict(exp=np.empty((n, 8)), log=np.empty((n, 7)), mul=np.empty((n, 8)), inv=np.empty((n, 8)), oplus=np.empty((n, 8)))
+    _chk(lib().ccm_sim3_debug_ops(n, _p(u), _p(a), _p(b), int(bool(fix_scale)), *[_p(out[k]) for k in ("exp", "log", "mul", "inv", "oplus")]))
+    return out
+
+
+def pgo_debug_edges(meas, si, sj, free_ij, fix_scale=False):
+    """ccm_pgo_debug_edges: the device's per-edge error (n,7) and Jacobians Ji, Jj (n,7,7); free_ij (n,2) != 0 marks a free side"""
+    m, a, b = [np.ascontiguousarray(v, np.float64).reshape(-1, 8) for v in (meas, si, sj)]
+    f = np.ascontiguousarray(free_ij, np.int32).reshape(-1, 2)
+    n = m.shape[0]
+    err = np.empty((n, 7)); Ji = np.empty((n, 7, 7)); Jj = np.empty((n, 7, 7))
+    _chk(lib().ccm_pgo_debug_edges(n, _p(m), _p(a), _p(b), _p(f), int(bool(fix_scale)), _p(err), _p(Ji), _p(Jj)))
+    return dict(err=err, Ji=Ji, Jj=Jj)
+
+
+PGO_PATH_KEYS = ("pcg_block", "pcg_agg", "pcg_nc", "coarse_used")
+
+
+def pgo_debug_system(p, lam, pcg_max_iter=0, pcg_tol=0.0):
+    """ccm_pgo_debug_system: one linearisation at p.sim3 and one PCG solve of (H + lam I) x = b with ccm_pgo_solve's set-up.
+    H is block CSR in free-vertex indices (rowptr (n+1,), col (nnzb,), H (nnzb,7,7), without lam)."""
+    arrs = dict(sim3=np.ascontiguousarray(p.sim3, np.float64), fixed=np.ascontiguousarray(p.fixed, np.uint8),
+                ei=np.ascontiguousarray(p.edge_i, np.int32), ej=np.ascontiguousarray(p.edge_j, np.int32),
+                meas=np.ascontiguousarray(p.meas, np.float64))
+    K, E = arrs["sim3"].shape[0], arrs["ei"].shape[0]
+    prob = PGOProblemC(K, E, _p(arrs["sim3"]), _p(arrs["fixed"]), _p(arrs["ei"]), _p(arrs["ej"]), _p(arrs["meas"]), int(p.fix_scale))
+    opt = PGOOptionsC(1, float(lam), pcg_max_iter, float(pcg_tol), None)
+    n = C.c_int32(); nnzb = C.c_int64()
+    f = lib().ccm_pgo_debug_system
+    f.argtypes = [C.c_void_p, C.c_void_p, C.c_double, C.c_void_p, C.c_void_p] + [C.c_void_p] * 10
+    _chk(f(C.byref(prob), C.byref(opt), lam, C.byref(n), C.byref(nnzb), *[None] * 10))
+    n, nnzb = n.value, nnzb.value
+    out = dict(vidx=np.empty(K, np.int32), rowptr=np.empty(n + 1, np.int32), col=np.empty(max(nnzb, 1), np.int32),
+               H=np.empty((max(nnzb, 1), 7, 7)), b=np.empty((n, 7)), Minv=np.empty((n, 7, 7)), x=np.empty((n, 7)),
+               chi2=np.empty(1), pcg=np.empty(4), paths=np.empty(4, np.int32))
+    _chk(f(C.byref(prob), C.byref(opt), lam, C.byref(C.c_int32()), C.byref(C.c_int64()),
+           *[_p(out[k]) for k in ("vidx", "rowptr", "col", "H", "b", "Minv", "x", "chi2", "pcg", "paths")]))
+    out["col"] = out["col"][:nnzb]; out["H"] = out["H"][:nnzb]
+    out.update(n=n, nnzb=nnzb, chi2=float(out["chi2"][0]), pcg_iters=int(out["pcg"][0]), pcg_relres=float(out["pcg"][1]),
+               pcg_flag=int(out["pcg"][2]), pcg_nC=int(out["pcg"][3]),
+               paths={k: int(v) for k, v in zip(PGO_PATH_KEYS, out["paths"])})
+    return out
+
+
 def hamming_matrix(A, B):
     A = np.ascontiguousarray(A, np.uint8).reshape(-1, 32); B = np.ascontiguousarray(B, np.uint8).reshape(-1, 32)
     D = np.empty((A.shape[0], B.shape[0]), np.uint16)

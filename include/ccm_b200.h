@@ -220,6 +220,26 @@ typedef struct ccm_pgo_result {
 
 int ccm_pgo_solve(const ccm_pgo_problem* p, const ccm_pgo_options* o, ccm_pgo_result* r);
 
+/* test-only entry points: the device code of ccm_pgo_solve on caller-chosen inputs (host buffers in and out).
+ * ccm_sim3_debug_ops: one thread per row runs s3_exp(u), s3_log(a), s3_mul(a, b), s3_inv(a) and s3_oplus(a, u, fix_scale)
+ * (Sim3 rows as in ccm_pgo_problem.sim3, updates u as 7-vectors omega, upsilon, sigma). */
+int ccm_sim3_debug_ops(int32_t n, const double* u /*n*7*/, const double* a /*n*8*/, const double* b /*n*8*/, int32_t fix_scale,
+                       double* exp_u /*n*8*/, double* log_a /*n*7*/, double* mul_ab /*n*8*/, double* inv_a /*n*8*/,
+                       double* oplus_u_a /*n*8*/);
+/* the per-edge linearisation of ccm_pgo_solve: error log(meas * si * sj^-1) and its central-difference Jacobians (row-major 7x7,
+ * J[r*7+d] = de_r/du_d); free_ij[2e], free_ij[2e+1] == 0 marks the side as fixed (its Jacobian is zero) */
+int ccm_pgo_debug_edges(int32_t n, const double* meas /*n*8*/, const double* si /*n*8*/, const double* sj /*n*8*/,
+                        const int32_t* free_ij /*n*2*/, int32_t fix_scale, double* err /*n*7*/, double* Ji /*n*49*/, double* Jj /*n*49*/);
+/* one linearisation at p->sim3 and one PCG solve of (H + lambda I) x = b, with the set-up, kernels and options of ccm_pgo_solve.
+ * Always writes n_free (free vertices with an edge) and nnzb (stored 7x7 blocks of H); vidx (K: free index or -1), rowptr (n+1),
+ * col (nnzb; full symmetric pattern, columns ascending, free-index space) and paths when given.  With H == NULL nothing runs on
+ * the device.  Otherwise H (nnzb*49, without lambda), b (n*7), Minv (n*49: inverses of the damped diagonal blocks), x (n*7),
+ * chi2 and pcg (4: iterations, relative residual, flag 0 converged / 1 max_iter / 2 breakdown, coarse size 7*nc or 0) are written.
+ * paths (4): PCG CTA size, coarse aggregate size, coarse nodes, coarse inverse used (1/0). */
+int ccm_pgo_debug_system(const ccm_pgo_problem* p, const ccm_pgo_options* o, double lambda, int32_t* n_free, int64_t* nnzb,
+                         int32_t* vidx, int32_t* rowptr, int32_t* col, double* H, double* b, double* Minv, double* x, double* chi2,
+                         double* pcg, int32_t* paths);
+
 /* ---- single-vertex optimisations ------------------------------------------------------------------------
  * ccm_pose_optimize replaces the g2o part of Optimizer::PoseOptimizationClient (cslam/src/Optimizer.cpp:215-347): one SE3
  * vertex, n unary EdgeSE3ProjectXYZOnlyPose, Huber sqrt(5.991), 4 x {estimate := Tcw, optimize(10), chi2 > 5.991 -> outlier},
