@@ -32,7 +32,8 @@ constexpr int kPatch = 31;
 
 __constant__ signed char c_pattern[1024];
 __constant__ int c_umax[16];
-__constant__ int c_blur_taps[7];
+
+struct BlurTaps { int k[7]; };  // per handle (ccm_orb_config::blur_2413), so handles of both tap sets can coexist
 
 struct Cell {            // one FAST cell of one pyramid level
   int level, img_off, img_w;
@@ -252,7 +253,8 @@ __device__ __forceinline__ int reflect101(int p, int n) {
   return p;
 }
 
-__global__ void __launch_bounds__(256) k_blur(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, int w, int h) {
+__global__ void __launch_bounds__(256) k_blur(const uint8_t* __restrict__ src, uint8_t* __restrict__ dst, int w, int h,
+                                              const BlurTaps taps) {
   __shared__ unsigned short rowpass[(16 + 6) * 32];  // 22 rows x 32 cols of horizontal sums (8.8 fixed point)
   const int bx = blockIdx.x * 32, by = blockIdx.y * 16;
   for (int i = threadIdx.x; i < 22 * 32; i += 256) {
@@ -262,7 +264,7 @@ __global__ void __launch_bounds__(256) k_blur(const uint8_t* __restrict__ src, u
     unsigned s = 0;
     if (x < w) {
 #pragma unroll
-      for (int k = -3; k <= 3; k++) s += (unsigned)c_blur_taps[k + 3] * src[(size_t)y * w + reflect101(x + k, w)];
+      for (int k = -3; k <= 3; k++) s += (unsigned)taps.k[k + 3] * src[(size_t)y * w + reflect101(x + k, w)];
     }
     rowpass[i] = (unsigned short)s;
   }
@@ -273,7 +275,7 @@ __global__ void __launch_bounds__(256) k_blur(const uint8_t* __restrict__ src, u
     if (x >= w || y >= h) continue;
     unsigned s = 0;
 #pragma unroll
-    for (int k = 0; k < 7; k++) s += (unsigned)c_blur_taps[k] * rowpass[(ty + k) * 32 + tx];
+    for (int k = 0; k < 7; k++) s += (unsigned)taps.k[k] * rowpass[(ty + k) * 32 + tx];
     dst[(size_t)y * w + x] = (uint8_t)min((s + 32768u) >> 16, 255u);
   }
 }
@@ -390,10 +392,15 @@ void divide_node(const QNode& n, const Cand* cand, QNode out[4]) {
   for (int q = 0; q < 4; q++) out[q].no_more = out[q].keys.size() == 1;
 }
 
+// number of root nodes of DistributeOctTree on a level whose bordered area is [minX, maxX) x [minY, maxY)
+int quadtree_roots(int minX, int maxX, int minY, int maxY) {
+  return (int)std::round(static_cast<float>(maxX - minX) / (maxY - minY));
+}
+
 std::vector<int> distribute(const Cand* cand, int n, int minX, int maxX, int minY, int maxY, int N) {
   std::vector<int> result;
   if (n == 0) return result;
-  const int nIni = (int)std::round(static_cast<float>(maxX - minX) / (maxY - minY));
+  const int nIni = quadtree_roots(minX, maxX, minY, maxY);
   CCM_REQUIRE(nIni >= 1, "ccm_orb_extract: image too tall for the reference's quadtree (nIni == 0)");
   const float hX = static_cast<float>(maxX - minX) / nIni;
   Quadtree t;
@@ -480,6 +487,7 @@ struct ccm_orb_handle {
   std::vector<int> cell_begin;  // first cell of each level (+ total)
   size_t pyr_bytes = 0;
   int ncells = 0, tile_cap = 0, max_per_cell = 0, max_cand = 0, max_kp = 0;
+  BlurTaps taps;
   DevBuf<uint8_t> pyr, blurred, desc;
   DevBuf<Cell> cells;
   DevBuf<LevelRef> levels;
@@ -545,8 +553,8 @@ void orb_build(ccm_orb_handle* h, const ccm_orb_config* cfg, int width, int heig
   }
   CCM_CUDA(cudaMemcpyToSymbolAsync(c_umax, umax, sizeof(umax), 0, cudaMemcpyHostToDevice, s));
   CCM_CUDA(cudaMemcpyToSymbolAsync(c_pattern, kOrbPattern, 1024, 0, cudaMemcpyHostToDevice, s));
-  static const int taps4[7] = {18, 34, 48, 56, 48, 34, 18}, taps2[7] = {18, 34, 49, 55, 49, 34, 18};
-  CCM_CUDA(cudaMemcpyToSymbolAsync(c_blur_taps, cfg->blur_2413 ? taps2 : taps4, sizeof(taps4), 0, cudaMemcpyHostToDevice, s));
+  static const BlurTaps taps4 = {{18, 34, 48, 56, 48, 34, 18}}, taps2 = {{18, 34, 49, 55, 49, 34, 18}};
+  h->taps = cfg->blur_2413 ? taps2 : taps4;
   // level geometry (ComputePyramid)
   h->lw.resize(nl); h->lh.resize(nl); h->loff.resize(nl);
   size_t off = 0;
@@ -624,14 +632,23 @@ void orb_build(ccm_orb_handle* h, const ccm_orb_config* cfg, int width, int heig
   h->cells.upload(cells.data(), cells.size(), s);
   h->cell_count.alloc(h->ncells); h->cell_off.alloc((size_t)h->ncells + 1);
   h->cell_out.alloc((size_t)out_off);
-  h->max_cand = std::max(10 * cfg->nfeatures, 20000);  // vToDistributeKeys.reserve(nfeatures*10)
-  h->max_cand = std::min(h->max_cand, out_off);
+  // The reference never caps the candidate list (vToDistributeKeys.reserve only reserves), so the gather buffers take every
+  // per-cell slot: out_off * sizeof(Cand) pinned and on the device, 7.2 MB each at 752x480 with the default configuration.
+  h->max_cand = out_off;
   h->cand.alloc(h->max_cand);
-  h->max_kp = cfg->nfeatures + 4 * nl + 64;
+  // Keypoint capacity: DistributeOctTree (S/ORBextractor.cpp:707-931) keeps one keypoint per node.  On a level with quota N
+  // it starts from nIni root nodes and its first pass splits every root holding more than one candidate, so that pass alone
+  // can leave 4 * nIni nodes whatever N is.  Every later full pass runs only if the node count plus three per splittable
+  // node is at most N, so it cannot exceed N.  The node-by-node loop splits only while fewer than N nodes exist, and one
+  // split adds at most three, so it stops below N + 3.  Hence at most max(4 * nIni, N + 3) keypoints per level.
+  h->max_kp = 0;
+  for (int l = 0; l < nl; l++)
+    h->max_kp += std::max(4 * quadtree_roots(kEdge - 3, h->lw[l] - kEdge + 3, kEdge - 3, h->lh[l] - kEdge + 3), h->n_per_level[l] + 3);
   h->kp_in.alloc(h->max_kp); h->desc.alloc((size_t)h->max_kp * 32);
   CCM_CUDA(cudaMallocHost((void**)&h->h_img, (size_t)width * height));
   CCM_CUDA(cudaMallocHost((void**)&h->h_cand, sizeof(Cand) * (size_t)h->max_cand));
   CCM_CUDA(cudaMallocHost((void**)&h->h_total, sizeof(int) * 4));
+  h->h_total[0] = 0;  // ccm_orb_debug_candidates before the first extract reports an empty list
   CCM_CUDA(cudaMallocHost((void**)&h->h_kp, sizeof(KpIn) * (size_t)h->max_kp));
   CCM_CUDA(cudaMallocHost((void**)&h->h_desc, (size_t)h->max_kp * 32));
   const size_t smem = ((size_t)h->tile_cap + 15) / 16 * 16 + 3 * (size_t)h->tile_cap + 16;
@@ -665,14 +682,15 @@ void orb_extract(ccm_orb_handle* h, const uint8_t* img, int stride, ccm_keypoint
   // the blur of every level overlaps with the host-side quadtree below
   for (int l = 0; l < nl; l++) {
     dim3 g(div_up(h->lw[l], 32), div_up(h->lh[l], 16));
-    k_blur<<<g, 256, 0, s>>>(h->pyr.p + h->loff[l], h->blurred.p + h->loff[l], h->lw[l], h->lh[l]);
+    k_blur<<<g, 256, 0, s>>>(h->pyr.p + h->loff[l], h->blurred.p + h->loff[l], h->lw[l], h->lh[l], h->taps);
     CCM_LAUNCHED();
   }
   // copy an optimistic prefix of the candidates together with the count, top up if there are more
   const int first = std::min(h->max_cand, 16384);
   CCM_CUDA(cudaMemcpyAsync(h->h_cand, h->cand.p, sizeof(Cand) * (size_t)first, cudaMemcpyDeviceToHost, s));
   CCM_CUDA(cudaStreamSynchronize(s));
-  const int total = std::min(h->h_total[0], h->max_cand);
+  const int total = h->h_total[0];
+  CCM_REQUIRE(total <= h->max_cand, "internal: more FAST candidates than per-cell slots");
   if (total > first) {
     CCM_CUDA(cudaMemcpyAsync(h->h_cand + first, h->cand.p + first, sizeof(Cand) * (size_t)(total - first), cudaMemcpyDeviceToHost, s));
     CCM_CUDA(cudaStreamSynchronize(s));
@@ -708,8 +726,11 @@ void orb_extract(ccm_orb_handle* h, const uint8_t* img, int stride, ccm_keypoint
       out.push_back(kp);
     }
   }
-  int n = (int)out.size();
-  CCM_REQUIRE(n <= h->max_kp, "internal: more keypoints than reserved");
+  const int n = (int)out.size();
+  CCM_REQUIRE(n <= h->max_kp, "internal: more keypoints than ccm_orb_max_keypoints");
+  *n_out = n;
+  CCM_REQUIRE(n <= max_kp, "ccm_orb_extract: " + std::to_string(n) + " keypoints, max_kp is " + std::to_string(max_kp) +
+                               " (size kps and desc with ccm_orb_max_keypoints)");
   if (n > 0) {
     memcpy(h->h_kp, kin.data(), sizeof(KpIn) * (size_t)n);
     CCM_CUDA(cudaMemcpyAsync(h->kp_in.p, h->h_kp, sizeof(KpIn) * (size_t)n, cudaMemcpyHostToDevice, s));
@@ -718,10 +739,8 @@ void orb_extract(ccm_orb_handle* h, const uint8_t* img, int stride, ccm_keypoint
     CCM_CUDA(cudaMemcpyAsync(h->h_desc, h->desc.p, (size_t)n * 32, cudaMemcpyDeviceToHost, s));
     CCM_CUDA(cudaStreamSynchronize(s));
   }
-  const int ncopy = std::min(n, max_kp);
-  for (int i = 0; i < ncopy; i++) kps[i] = out[i];
-  if (desc && ncopy) memcpy(desc, h->h_desc, (size_t)ncopy * 32);
-  *n_out = ncopy;
+  for (int i = 0; i < n; i++) kps[i] = out[i];
+  if (desc && n) memcpy(desc, h->h_desc, (size_t)n * 32);
 }
 
 }  // namespace
@@ -744,8 +763,15 @@ extern "C" int ccm_orb_create(const ccm_orb_config* cfg, int32_t width, int32_t 
 extern "C" int ccm_orb_extract(ccm_orb_handle* h, const uint8_t* img, int32_t stride, ccm_keypoint* kps, int32_t max_kp,
                                int32_t* n, uint8_t* desc) {
   return guarded([&] {
-    CCM_REQUIRE(h && img && kps && n && stride >= h->width, "ccm_orb_extract: bad argument");
+    CCM_REQUIRE(h && img && kps && n && max_kp >= 0 && stride >= h->width, "ccm_orb_extract: bad argument");
     orb_extract(h, img, stride, kps, max_kp, n, desc);
+  });
+}
+
+extern "C" int ccm_orb_max_keypoints(const ccm_orb_handle* h, int32_t* n) {
+  return guarded([&] {
+    CCM_REQUIRE(h && n, "ccm_orb_max_keypoints: null argument");
+    *n = h->max_kp;
   });
 }
 
@@ -753,7 +779,7 @@ extern "C" int ccm_orb_extract(ccm_orb_handle* h, const uint8_t* img, int32_t st
 extern "C" int ccm_orb_debug_candidates(ccm_orb_handle* h, float* xys, int32_t* level, int32_t max_out, int32_t* n) {
   return guarded([&] {
     CCM_REQUIRE(h && n, "null argument");
-    const int total = std::min(h->h_total[0], h->max_cand);
+    const int total = h->h_total[0];
     *n = total;
     for (int i = 0; i < std::min(total, max_out); i++) {
       xys[3 * i] = h->h_cand[i].x; xys[3 * i + 1] = h->h_cand[i].y; xys[3 * i + 2] = (float)h->h_cand[i].score;
@@ -772,6 +798,16 @@ extern "C" int ccm_orb_get_level(ccm_orb_handle* h, int32_t level, uint8_t* out,
       CCM_CUDA(cudaMemcpyAsync(out, h->pyr.p + h->loff[level], (size_t)h->lw[level] * h->lh[level], cudaMemcpyDeviceToHost, h->stream));
       CCM_CUDA(cudaStreamSynchronize(h->stream));
     }
+  });
+}
+
+// debug: the blurred pyramid level the descriptors of the last ccm_orb_extract call sampled
+extern "C" int ccm_orb_debug_blurred(ccm_orb_handle* h, int32_t level, uint8_t* out) {
+  return guarded([&] {
+    CCM_REQUIRE(h && out && level >= 0 && level < h->cfg.nlevels, "ccm_orb_debug_blurred: bad argument");
+    CCM_CUDA(cudaSetDevice(h->device));
+    CCM_CUDA(cudaMemcpyAsync(out, h->blurred.p + h->loff[level], (size_t)h->lw[level] * h->lh[level], cudaMemcpyDeviceToHost, h->stream));
+    CCM_CUDA(cudaStreamSynchronize(h->stream));
   });
 }
 

@@ -26,7 +26,9 @@ class ORBextractor:
         self.width, self.height, self.nlevels = width, height, nlevels
         self._h = C.c_void_p()
         _chk(lib().ccm_orb_create(C.byref(self.cfg), width, height, C.byref(self._h)))
-        self.max_kp = nfeatures + 4 * nlevels + 64
+        n = C.c_int32()
+        _chk(lib().ccm_orb_max_keypoints(self._h, C.byref(n)))
+        self.max_kp = n.value
 
     def __call__(self, image):
         """operator()(image, mask, keypoints, descriptors): returns (keypoints structured array, descriptors N x 32 u8)."""

@@ -308,13 +308,21 @@ typedef struct ccm_keypoint {  /* cv::KeyPoint fields the reference reads */
 
 typedef struct ccm_orb_handle ccm_orb_handle;
 int ccm_orb_create(const ccm_orb_config* cfg, int32_t width, int32_t height, ccm_orb_handle** out);
-/* extract: kps capacity max_kp; returns count in *n; desc = n*32 bytes */
+/* the most keypoints one extract call on this handle can return: sum over the levels of max(4 * nIni, quota + 3), where nIni
+ * is the number of root nodes of the level's quadtree; size kps (and desc, 32 bytes each) with it */
+int ccm_orb_max_keypoints(const ccm_orb_handle* h, int32_t* n);
+/* extract: kps capacity max_kp; returns count in *n; desc = n*32 bytes.  When the count exceeds max_kp the call fails with
+ * CCM_ERR_INVALID, *n holds the count and kps / desc are not written. */
 int ccm_orb_extract(ccm_orb_handle* h, const uint8_t* img, int32_t stride, ccm_keypoint* kps, int32_t max_kp,
                     int32_t* n, uint8_t* desc);
 /* pyramid level readback (mvImagePyramid[level], public member of the reference class) */
 int ccm_orb_get_level(ccm_orb_handle* h, int32_t level, uint8_t* out, int32_t* w, int32_t* hgt);
-/* test hook: FAST candidates of the last extract call before the quadtree (3 floats each: x, y relative to the 16 px border, score) */
+/* test hook: FAST candidates of the last extract call before the quadtree (3 floats each: x, y relative to the 16 px border, score);
+ * *n = the full count, the first min(*n, max_out) are written */
 int ccm_orb_debug_candidates(ccm_orb_handle* h, float* xys, int32_t* level, int32_t max_out, int32_t* n);
+/* test hook: blurred pyramid level of the last extract call (GaussianBlur 7x7 that the descriptors sample), width x height bytes
+ * as ccm_orb_get_level reports them */
+int ccm_orb_debug_blurred(ccm_orb_handle* h, int32_t level, uint8_t* out);
 void ccm_orb_destroy(ccm_orb_handle* h);
 
 /* ---- Hamming matching ----------------------------------------------------------------------------------

@@ -1,6 +1,8 @@
 // ccm_orb_double.cpp — link-time stand-in for the device ORB extractor behind shim/ORBextractor_shim.cpp (TEST INFRASTRUCTURE, NOT PRODUCT).
-// ccm_orb_create / extract / get_level on top of the CPU oracle, so that the shim's own code (scale tables, handle cache, keypoint and
+// ccm_orb_create / max_keypoints / extract / get_level on top of the CPU oracle, so that the shim's own code (scale tables, handle cache, keypoint and
 // descriptor marshalling, the public mvImagePyramid) can run without a GPU.  Linked only into oracle/_ref/libextractor_shim.so.
+#include <algorithm>
+#include <cmath>
 #include <cstdint>
 #include <cstring>
 #include <vector>
@@ -28,12 +30,31 @@ int ccm_orb_create(const ccm_orb_config* c, int32_t width, int32_t height, ccm_o
   *out = h;
   return CCM_OK;
 }
+// the device library's bound (orb.cu): per level max(4 * nIni, quota + 3), nIni = root nodes of the level's quadtree
+int ccm_orb_max_keypoints(const ccm_orb_handle* h, int32_t* n) {
+  const int L = h->cfg.nlevels;
+  std::vector<int> npl(L), umax(16), wh(2 * L);
+  orc_orb_tables(&h->cfg, h->w, h->h, npl.data(), umax.data(), wh.data());
+  int cap = 0;
+  for (int l = 0; l < L; l++) {
+    const int border = 2 * (19 - 3);             // the quadtree spans the level less EDGE_THRESHOLD - 3 on each side
+    const int nIni = (int)std::round(static_cast<float>(wh[2 * l] - border) / (wh[2 * l + 1] - border));
+    cap += std::max(4 * nIni, npl[l] + 3);
+  }
+  *n = cap;
+  return CCM_OK;
+}
 int ccm_orb_extract(ccm_orb_handle* h, const uint8_t* img, int32_t stride, ccm_keypoint* kps, int32_t max_kp, int32_t* n, uint8_t* desc) {
-  std::vector<orc_keypoint> k(max_kp);
+  int cap = 0;
+  ccm_orb_max_keypoints(h, &cap);
+  std::vector<orc_keypoint> k(cap);
+  std::vector<uint8_t> d((size_t)cap * 32);
   int cnt = 0;
-  orc_orb_extract(img, h->w, h->h, stride, &h->cfg, k.data(), max_kp, &cnt, desc);
-  for (int i = 0; i < cnt; i++) kps[i] = ccm_keypoint{k[i].x, k[i].y, k[i].size, k[i].angle, k[i].response, k[i].octave};
+  orc_orb_extract(img, h->w, h->h, stride, &h->cfg, k.data(), cap, &cnt, d.data());
   *n = cnt;
+  if (cnt > max_kp) return CCM_ERR_INVALID;   // as the device library: refuse, write nothing
+  for (int i = 0; i < cnt; i++) kps[i] = ccm_keypoint{k[i].x, k[i].y, k[i].size, k[i].angle, k[i].response, k[i].octave};
+  if (desc) std::memcpy(desc, d.data(), (size_t)cnt * 32);
   // ComputePyramid (S/ORBextractor.cpp:1280-1304): level l is level l-1 resized, INTER_LINEAR
   const int L = h->cfg.nlevels;
   std::vector<int> npl(L), umax(16);

@@ -45,7 +45,8 @@ void ORBextractor::operator()(cv::InputArray _image, cv::InputArray /*_mask*/, s
     }
     h = it->second;
   }
-  const int cap = nfeatures + 4 * nlevels + 64;
+  int cap = 0;
+  if (ccm_orb_max_keypoints(h, &cap) != CCM_OK) throw estd::infrastructure_ex();
   std::vector<ccm_keypoint> kps(cap);
   cv::Mat desc(cap, 32, CV_8U);
   int n = 0;

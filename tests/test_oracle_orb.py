@@ -7,7 +7,7 @@ import pytest
 
 cv2 = pytest.importorskip("cv2")
 
-from ccm_slam_b200.synth_images import make_image
+from ccm_slam_b200.synth_images import make_image, make_noise
 
 
 @pytest.fixture(scope="module")
@@ -30,6 +30,23 @@ def test_resize_chain_matches_cv2(oracle, img):
         got = oracle.resize_linear_u8(cur, w, h)
         assert np.array_equal(got, ref)
         cur = ref
+
+
+@pytest.mark.parametrize("w,h,sf,nl", [(752, 480, 1.1, 12), (752, 480, 1.5, 5), (1024, 768, 2.0, 4), (1024, 768, 1.2, 8), (641, 479, 1.2, 8),
+                                       (1280, 240, 1.2, 8), (221, 221, 1.2, 8)])
+@pytest.mark.parametrize("frame", ["make_image", "noise"])
+def test_pyramid_and_blur_of_other_scales_and_sizes_match_cv2(oracle, w, h, sf, nl, frame):
+    """every level of the chained resize and its 7x7 blur, for the scale factors and frame sizes the device tests sweep"""
+    _, _, wh = oracle.orb_tables(oracle.orb_cfg(scale_factor=sf, nlevels=nl), w, h)
+    cur = make_image(4, w, h) if frame == "make_image" else make_noise(3, w, h, 1.0)
+    for l in range(nl):
+        w_l, h_l = int(wh[l, 0]), int(wh[l, 1])
+        if l:
+            ref = cv2.resize(cur, (w_l, h_l), interpolation=cv2.INTER_LINEAR)
+            assert np.array_equal(oracle.resize_linear_u8(cur, w_l, h_l), ref), l
+            cur = ref
+        blur = cv2.GaussianBlur(cur, (7, 7), 2, 2, borderType=cv2.BORDER_REFLECT_101)
+        assert np.array_equal(oracle.gaussian_blur7(cur), blur), l
 
 
 def test_gaussian_blur_matches_cv2(oracle, img):

@@ -12,7 +12,7 @@ monotone-allocator behaviour (DESIGN.md §3).  Skipped where neither /root/refer
 import numpy as np
 import pytest
 
-from ccm_slam_b200.synth_images import make_image
+from ccm_slam_b200.synth_images import make_image, make_noise
 
 FIELDS = ("x", "y", "size", "angle", "response", "octave")
 
@@ -54,6 +54,24 @@ def test_degenerate_images(ref):
     assert _same(ref.orb_extract(low), ref.ref_orb_extract(low))
     noise = rng.integers(0, 256, size=(240, 376), dtype=np.uint8)                        # far more corners than the quota
     assert _same(ref.orb_extract(noise), ref.ref_orb_extract(noise))
+
+
+@pytest.mark.parametrize("sigma", [0.0, 0.7, 1.0, 1.5])
+def test_textured_frames(ref, sigma):
+    """752x480 white and smoothed noise: 40 000 - 80 000 FAST candidates, every level far above its quota"""
+    img = make_noise(7, 752, 480, sigma)
+    got, want = ref.orb_extract(img), ref.ref_orb_extract(img)
+    assert len(want[0]) > 1000 and _same(got, want)
+
+
+@pytest.mark.parametrize("nfeatures", [8, 100])
+def test_wide_frames_with_small_quotas(ref, nfeatures):
+    """1280x240: the first quadtree split alone leaves more keypoints than the quota"""
+    c = ref.orb_cfg(nfeatures=nfeatures)
+    for img in (make_noise(1, 1280, 240), make_image(6, 1280, 240)):
+        got, want = ref.orb_extract(img, c), ref.ref_orb_extract(img, c)
+        assert _same(got, want)
+    assert len(want[0]) > nfeatures + 96
 
 
 def test_the_reference_itself_depends_on_the_allocator(ref):

@@ -11,7 +11,7 @@ import os
 import numpy as np
 import pytest
 
-from ccm_slam_b200.synth_images import make_image
+from ccm_slam_b200.synth_images import make_image, make_noise
 
 SO = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "oracle", "_ref", "libextractor_shim.so")
 
@@ -23,11 +23,25 @@ def xlib(oracle):
     return C.CDLL(SO)
 
 
-@pytest.mark.parametrize("seed,w,h,nfeat,nlev,sf", [(0, 752, 480, 1000, 8, 1.2), (3, 376, 240, 500, 6, 1.2), (5, 640, 480, 1500, 8, 1.3)])
+def _max_keypoints(xlib, cfg, w, h):
+    """ccm_orb_max_keypoints of the library the shim links against"""
+    handle = C.c_void_p(); cap = C.c_int32()
+    assert xlib.ccm_orb_create(C.byref(cfg), w, h, C.byref(handle)) == 0
+    try:
+        assert xlib.ccm_orb_max_keypoints(handle, C.byref(cap)) == 0
+    finally:
+        xlib.ccm_orb_destroy(handle)
+    return cap.value
+
+
+# (1280, 240, 8 features): each level's quadtree starts from 6 to 9 roots and its first split can leave four keypoints per
+# root whatever the quota; white noise gives 228 keypoints there
+@pytest.mark.parametrize("seed,w,h,nfeat,nlev,sf", [(0, 752, 480, 1000, 8, 1.2), (3, 376, 240, 500, 6, 1.2), (5, 640, 480, 1500, 8, 1.3),
+                                                    ("noise", 1280, 240, 8, 8, 1.2)])
 def test_extractor_shim_matches_reference_class(xlib, oracle, seed, w, h, nfeat, nlev, sf):
-    img = make_image(seed, w, h)
+    img = make_noise(1, w, h) if seed == "noise" else make_image(seed, w, h)
     cfg = oracle.orb_cfg(nfeatures=nfeat, nlevels=nlev, scale_factor=sf, blur_2413=1)      # the stand-in reports OpenCV 2.x: the 2.4.13 blur taps
-    cap = nfeat + 4 * nlev + 64
+    cap = _max_keypoints(xlib, cfg, w, h)
     kps = np.zeros(cap, oracle.KP_DTYPE); desc = np.zeros((cap, 32), np.uint8); tables = np.zeros((nlev, 4), np.float32)
     pyr = np.zeros(w * h * 4, np.uint8); wh = np.zeros((nlev, 2), np.int32); get = np.zeros(2, np.int32)
     p = lambda a: a.ctypes.data_as(C.c_void_p)
