@@ -413,33 +413,28 @@ class Sim3OptResultC(C.Structure):
     _fields_ = [("S12", C.c_double * 8), ("n_inliers", C.c_int32), ("inlier", C.c_void_p)]
 
 
-def pose_optimize(problems):
-    """Optimizer::PoseOptimizationClient for a batch of frames.  problems: list of dict(Tcw0, Xw, uv, inv_sigma2, intr)
-    (ccm_slam_b200.synth.make_pose_opt layout).  Returns a list of (Tcw (7,), outlier (n,) u8, n_inliers)."""
+def _pose_probs(problems, state_key="Tcw0"):
     B = len(problems)
     probs = (PoseOptProblemC * max(B, 1))(); res = (PoseOptResultC * max(B, 1))()
     keep = []
     for b, d in enumerate(problems):
-        a = dict(T=np.ascontiguousarray(d["Tcw0"], np.float64), X=np.ascontiguousarray(d["Xw"], np.float32).reshape(-1, 3),
+        a = dict(T=np.ascontiguousarray(d[state_key], np.float64), X=np.ascontiguousarray(d["Xw"], np.float32).reshape(-1, 3),
                  uv=np.ascontiguousarray(d["uv"], np.float32).reshape(-1, 2), w=np.ascontiguousarray(d["inv_sigma2"], np.float32))
         n = a["X"].shape[0]
         a["out"] = np.zeros(max(n, 1), np.uint8)
         keep.append(a)
         probs[b] = PoseOptProblemC(n, _p(a["T"]), _p(a["X"]), _p(a["uv"]), _p(a["w"]), *[float(v) for v in d["intr"]])
         res[b].outlier = _p(a["out"])
-    _chk(lib().ccm_pose_optimize(probs, B, res))
-    return [(np.array(res[b].Tcw[:]), keep[b]["out"][:keep[b]["X"].shape[0]], int(res[b].n_inliers)) for b in range(B)]
+    return probs, res, keep
 
 
-def sim3_optimize(problems):
-    """Optimizer::OptimizeSim3 for a batch of keyframe pairs.  problems: list of dict(S12_0, P1c, P2c, uv1, uv2, w1, w2, K1, K2,
-    th2, fix_scale) (synth.make_sim3_opt layout).  Returns a list of (S12 (8,), inlier (n,) u8, n_inliers)."""
+def _sim3_probs(problems, state_key="S12_0"):
     B = len(problems)
     probs = (Sim3OptProblemC * max(B, 1))(); res = (Sim3OptResultC * max(B, 1))()
     keep = []
     f32 = lambda x, c: np.ascontiguousarray(x, np.float32).reshape(-1, c) if c else np.ascontiguousarray(x, np.float32)
     for b, d in enumerate(problems):
-        a = dict(S=np.ascontiguousarray(d["S12_0"], np.float64), P1=f32(d["P1c"], 3), P2=f32(d["P2c"], 3), u1=f32(d["uv1"], 2),
+        a = dict(S=np.ascontiguousarray(d[state_key], np.float64), P1=f32(d["P1c"], 3), P2=f32(d["P2c"], 3), u1=f32(d["uv1"], 2),
                  u2=f32(d["uv2"], 2), w1=f32(d["w1"], 0), w2=f32(d["w2"], 0))
         n = a["P1"].shape[0]
         a["inl"] = np.zeros(max(n, 1), np.uint8)
@@ -448,8 +443,69 @@ def sim3_optimize(problems):
                                    (C.c_float * 4)(*[float(v) for v in d["K1"]]), (C.c_float * 4)(*[float(v) for v in d["K2"]]),
                                    float(d["th2"]), int(bool(d["fix_scale"])))
         res[b].inlier = _p(a["inl"])
-    _chk(lib().ccm_sim3_optimize(probs, B, res))
-    return [(np.array(res[b].S12[:]), keep[b]["inl"][:keep[b]["P1"].shape[0]], int(res[b].n_inliers)) for b in range(B)]
+    return probs, res, keep
+
+
+SINGLE_TRACE_CALL = 7 + 10 * 7     # CCM_SINGLE_TRACE_HEAD + CCM_SINGLE_TRACE_ITERS * CCM_SINGLE_TRACE_COLS
+SINGLE_TRACE_CALLS = {"pose": 4, "sim3": 2}
+
+
+def pose_optimize(problems, trace=False):
+    """Optimizer::PoseOptimizationClient for a batch of frames.  problems: list of dict(Tcw0, Xw, uv, inv_sigma2, intr)
+    (ccm_slam_b200.synth.make_pose_opt layout).  Returns a list of (Tcw (7,), outlier (n,) u8, n_inliers); with trace=True
+    (ccm_pose_optimize_traced, test only) each tuple also carries the LM trace (4, SINGLE_TRACE_CALL)."""
+    B = len(problems)
+    probs, res, keep = _pose_probs(problems)
+    if trace:
+        tr = np.empty((max(B, 1), SINGLE_TRACE_CALLS["pose"], SINGLE_TRACE_CALL))
+        _chk(lib().ccm_pose_optimize_traced(probs, B, res, _p(tr)))
+    else:
+        _chk(lib().ccm_pose_optimize(probs, B, res))
+    return [(np.array(res[b].Tcw[:]), keep[b]["out"][:keep[b]["X"].shape[0]], int(res[b].n_inliers)) + ((tr[b],) if trace else ())
+            for b in range(B)]
+
+
+def sim3_optimize(problems, trace=False):
+    """Optimizer::OptimizeSim3 for a batch of keyframe pairs.  problems: list of dict(S12_0, P1c, P2c, uv1, uv2, w1, w2, K1, K2,
+    th2, fix_scale) (synth.make_sim3_opt layout).  Returns a list of (S12 (8,), inlier (n,) u8, n_inliers); with trace=True
+    (ccm_sim3_optimize_traced, test only) each tuple also carries the LM trace (2, SINGLE_TRACE_CALL)."""
+    B = len(problems)
+    probs, res, keep = _sim3_probs(problems)
+    if trace:
+        tr = np.empty((max(B, 1), SINGLE_TRACE_CALLS["sim3"], SINGLE_TRACE_CALL))
+        _chk(lib().ccm_sim3_optimize_traced(probs, B, res, _p(tr)))
+    else:
+        _chk(lib().ccm_sim3_optimize(probs, B, res))
+    return [(np.array(res[b].S12[:]), keep[b]["inl"][:keep[b]["P1"].shape[0]], int(res[b].n_inliers)) + ((tr[b],) if trace else ())
+            for b in range(B)]
+
+
+def single_debug_system(kind, problems, states, active, robust, delta, lam):
+    """ccm_pose_debug_system (kind "pose", D = 6) / ccm_sim3_debug_system ("sim3", D = 7): per problem b, at states[b], with the
+    per-edge masks active[b], robust[b] (n / 2n entries), Huber delta[b] and lambda lam[b]: one system build and one damped solve
+    with the optimiser's device functions.  Returns per problem dict(err (E,2), J (E,2,D), H (D,D), b (D,), chi2, x (D,), solved)."""
+    D, per = (6, 1) if kind == "pose" else (7, 2)
+    key = "Tcw0" if kind == "pose" else "S12_0"
+    probs_l = [{"th2": 0.0, **d, key: np.asarray(s, np.float64)} for d, s in zip(problems, states)]   # th2 is not read here
+    probs, _, keep = (_pose_probs if kind == "pose" else _sim3_probs)(probs_l)
+    B = len(problems)
+    ne = [per * (k["X"] if kind == "pose" else k["P1"]).shape[0] for k in keep]
+    tot = sum(ne)
+    act = np.ascontiguousarray(np.concatenate([np.asarray(a, np.uint8).ravel() for a in active]) if B else np.zeros(0, np.uint8), np.uint8)
+    rob = np.ascontiguousarray(np.concatenate([np.asarray(a, np.uint8).ravel() for a in robust]) if B else np.zeros(0, np.uint8), np.uint8)
+    assert act.size == tot and rob.size == tot
+    dl = np.ascontiguousarray(np.stack([np.asarray(delta, np.float64), np.asarray(lam, np.float64)], 1) if B else np.zeros((1, 2)))
+    err = np.empty((max(tot, 1), 2)); J = np.empty((max(tot, 1), 2, D)); ns = D * D + 2 * D + 1
+    sys_ = np.empty((max(B, 1), ns)); sol = np.empty(max(B, 1), np.int32)
+    f = lib().ccm_pose_debug_system if kind == "pose" else lib().ccm_sim3_debug_system
+    _chk(f(probs, B, _p(act), _p(rob), _p(dl), _p(err), _p(J), _p(sys_), _p(sol)))
+    out, o = [], 0
+    for b in range(B):
+        s = sys_[b]
+        out.append(dict(err=err[o:o + ne[b]].copy(), J=J[o:o + ne[b]].copy(), H=s[:D * D].reshape(D, D).copy(), b=s[D * D:D * D + D].copy(),
+                        chi2=float(s[D * D + D]), x=s[D * D + D + 1:].copy(), solved=bool(sol[b])))
+        o += ne[b]
+    return out
 
 
 def _map_update_args(sc):

@@ -288,6 +288,33 @@ typedef struct ccm_sim3_opt_result {
 } ccm_sim3_opt_result;
 int ccm_sim3_optimize(const ccm_sim3_opt_problem* probs, int32_t batch, ccm_sim3_opt_result* res);
 
+/* test-only entry points: the device code of ccm_pose_optimize / ccm_sim3_optimize on caller-chosen inputs.
+ * ccm_{pose,sim3}_optimize_traced: the same protocol as the product entry points (same results), recording g2o's Levenberg
+ * protocol in `trace`: per problem CCM_SINGLE_TRACE_{POSE,SIM3}_CALLS optimize() calls of CCM_SINGLE_TRACE_HEAD +
+ * CCM_SINGLE_TRACE_ITERS * CCM_SINGLE_TRACE_COLS doubles each.  Header: end (0 iteration limit, 1 ten rejected trials,
+ * 2 rho == 0, 3 three iterations without gain, -1 no active edge), iterations, iteration limit of the call, chi2 of the cached
+ * edge errors the classification after the call reads, chi2 of fresh errors at the estimate over the same edges, number of those
+ * edges whose cached error is not bit-identical to the fresh one, edges (pose) / pairs (Sim3) the classification rejects.  Row per LM iteration: iniChi, lambda at its
+ * start, trials, rho of the last trial, currentChi at its end, accepted (1/0), failed Cholesky factorisations.  NaN where a call
+ * or an iteration did not happen. */
+#define CCM_SINGLE_TRACE_ITERS 10
+#define CCM_SINGLE_TRACE_COLS 7
+#define CCM_SINGLE_TRACE_HEAD 7
+#define CCM_SINGLE_TRACE_POSE_CALLS 4
+#define CCM_SINGLE_TRACE_SIM3_CALLS 2
+int ccm_pose_optimize_traced(const ccm_pose_opt_problem* probs, int32_t batch, ccm_pose_opt_result* res, double* trace);
+int ccm_sim3_optimize_traced(const ccm_sim3_opt_problem* probs, int32_t batch, ccm_sim3_opt_result* res, double* trace);
+/* ccm_{pose,sim3}_debug_system: per problem, at the state probs[b].Tcw / .S12, with the edge masks active / robust (edges of all
+ * problems back to back: n per pose problem, 2n per Sim3 problem, edge 2i the forward and 2i+1 the inverse edge of pair i) and
+ * delta_lambda[2b] = Huber delta, [2b+1] = lambda: one system build and one damped solve with the optimiser's device functions.
+ * err (2 per edge) and J (2 x D row-major per edge, D = 6 / 7) for every edge; sys per problem = H (D*D, without lambda), b (D),
+ * robust chi2 of the active edges, x (D) of (H + lambda I) x = b; solved[b] = 1, or 0 with x = 0 when a pivot is not positive.
+ * th2 of a Sim3 problem is not read. */
+int ccm_pose_debug_system(const ccm_pose_opt_problem* probs, int32_t batch, const uint8_t* active, const uint8_t* robust,
+                          const double* delta_lambda, double* err, double* J, double* sys, int32_t* solved);
+int ccm_sim3_debug_system(const ccm_sim3_opt_problem* probs, int32_t batch, const uint8_t* active, const uint8_t* robust,
+                          const double* delta_lambda, double* err, double* J, double* sys, int32_t* solved);
+
 /* ---- ORB front end ------------------------------------------------------------------------------------
  * ccm_orb_* replace ORBextractor::operator() (cslam/src/ORBextractor.cpp:1216-1278) and its helpers
  * (ComputePyramid :1280-1304, ComputeKeyPointsOctTree :933-1024, IC_Angle :68-95, computeOrbDescriptor :100-316);

@@ -151,6 +151,10 @@ typedef struct {
 } orc_sim3_opt_problem;
 /* Optimizer::OptimizeSim3 (S/Optimizer.cpp:861-1056); returns nIn (0 and S12 untouched when fewer than 10 pairs survive) */
 int orc_sim3_optimize(const orc_sim3_opt_problem* p, double* S12_out /*8*/, uint8_t* inlier /*n: vpMatches1[i] kept*/);
+/* the same two protocols, recording every optimize() call in `trace` (4 / 2 calls of 7 + 10 * 7 doubles, the layout of
+ * ccm_pose_optimize_traced in include/ccm_b200.h); the results are those of orc_pose_optimize / orc_sim3_optimize */
+int orc_pose_opt_trace(const orc_pose_opt_problem* p, double* Tcw_out, uint8_t* outlier, double* trace /*4*77*/);
+int orc_sim3_opt_trace(const orc_sim3_opt_problem* p, double* S12_out, uint8_t* inlier, double* trace /*2*77*/);
 /* pieces: the quadratic form all edges build at a given estimate — H (DxD row-major), b (D), err (2 per edge; Sim3: edge 2i / 2i+1) */
 void orc_pose_opt_build(const orc_pose_opt_problem* p, const double* Tcw, int robust, double delta, double* H, double* b, double* err);
 void orc_sim3_opt_build(const orc_sim3_opt_problem* p, const double* S12, int robust, double delta, double* H, double* b, double* err);

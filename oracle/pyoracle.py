@@ -901,6 +901,23 @@ def sim3_optimize(S12, P1c, P2c, uv1, uv2, w1, w2, K1, K2, th2, fix_scale, fn=No
     return out, inl[:n], nin
 
 
+SINGLE_TRACE_CALL = 7 + 10 * 7     # header {end, iterations, limit, cached chi2, fresh chi2, stale edges, rejected} + 10 LM rows of 7
+
+
+def pose_opt_trace(Tcw, Xw, uv, inv_sigma2, intr):
+    """pose_optimize + the LM trace of its optimize() calls: (Tcw, outlier, n_inliers, trace (4, SINGLE_TRACE_CALL))"""
+    trace = np.empty((4, SINGLE_TRACE_CALL))
+    f = lambda prob, out, outl: lib().orc_pose_opt_trace(prob, out, outl, _p(trace))
+    return pose_optimize(Tcw, Xw, uv, inv_sigma2, intr, fn=f) + (trace,)
+
+
+def sim3_opt_trace(S12, P1c, P2c, uv1, uv2, w1, w2, K1, K2, th2, fix_scale):
+    """sim3_optimize + the LM trace of its two optimize() calls: (S12, inlier, n_inliers, trace (2, SINGLE_TRACE_CALL))"""
+    trace = np.empty((2, SINGLE_TRACE_CALL))
+    f = lambda prob, out, inl: lib().orc_sim3_opt_trace(prob, out, inl, _p(trace))
+    return sim3_optimize(S12, P1c, P2c, uv1, uv2, w1, w2, K1, K2, th2, fix_scale, fn=f) + (trace,)
+
+
 # ---- the two single-vertex optimisations run by the reference's LM driver over the reference's vertices / edges (oracle/ref_single_full_wrap.cpp)
 _REF_SINGLE = None
 

@@ -25,6 +25,11 @@
 namespace {
 using namespace orc;
 
+// LM trace of one optimize() call: {end, iterations, iteration limit, cached chi2, fresh chi2, stale edges, rejected} +
+// TRACE_ITERS rows of TRACE_COLS
+// (the layout of the device's trace, include/ccm_b200.h)
+constexpr int TRACE_ITERS = 10, TRACE_COLS = 7, TRACE_HEAD = 7, TRACE_CALL = TRACE_HEAD + TRACE_ITERS * TRACE_COLS;
+
 inline void huber1(double e, double delta, double rho[3]) {  // G/core/robust_kernel_impl.cpp:77-91
   const double dsqr = (double)(float)(delta * delta);  // float member, G/core/robust_kernel_impl.h:84
   if (e <= dsqr) {
@@ -154,6 +159,7 @@ struct Single {
   std::vector<uint8_t> active, robust;  // per edge: level 0 ; has a Huber kernel
   std::vector<double> err;              // cached _error of every edge (2 per edge)
   double delta = 0;
+  double* trace = nullptr;              // optional: the current call's trace slot (layout of ccm_single trace in ccm_b200.h)
 
   void oplus(const double* x) {
     if constexpr (D == 7) m.oplus_fs(est, x); else M::oplus(est, x);
@@ -196,9 +202,9 @@ struct Single {
   int optimize(int iterations) {
     bool any = false;
     for (int e = 0; e < m.n_edges(); e++) any = any || active[e];
-    if (!any) return -1;
+    if (!any) { if (trace) { trace[0] = -1; trace[1] = -1; trace[2] = iterations; } return -1; }
     double lambda = -1, ni = 2;
-    int n_bad = 0, done = 0;
+    int n_bad = 0, done = 0, end = 0;
     bool ok = true;
     for (int it = 0; it < iterations && ok; it++) {
       compute_active_errors();
@@ -212,6 +218,8 @@ struct Single {
         for (int i = 0; i < D; i++) maxd = std::max(std::fabs(H[i * D + i]), maxd);
         lambda = 1e-5 * maxd; ni = 2; n_bad = 0;
       }
+      const double lambda0 = lambda;
+      int nfail = 0;
       double rho = 0;
       int qmax = 0;
       do {
@@ -224,7 +232,7 @@ struct Single {
         oplus(x);
         compute_active_errors();
         tempChi = active_robust_chi2();
-        if (!ok2) tempChi = std::numeric_limits<double>::max();
+        if (!ok2) { tempChi = std::numeric_limits<double>::max(); nfail++; }
         rho = currentChi - tempChi;
         double scale = 0;
         for (int i = 0; i < D; i++) scale += x[i] * (lambda * x[i] + b[i]);
@@ -242,18 +250,40 @@ struct Single {
         }
         qmax++;
       } while (rho < 0 && qmax < 10);
+      if (trace && it < TRACE_ITERS) {
+        double* r = trace + TRACE_HEAD + it * TRACE_COLS;
+        r[0] = iniChi; r[1] = lambda0; r[2] = qmax; r[3] = rho; r[4] = currentChi; r[5] = (rho > 0 && std::isfinite(tempChi)) ? 1 : 0;
+        r[6] = nfail;
+      }
       done++;
-      if (qmax == 10 || rho == 0) { ok = false; continue; }
+      if (qmax == 10 || rho == 0) { ok = false; end = qmax == 10 ? 1 : 2; continue; }
       if ((iniChi - currentChi) * 1e3 < iniChi) n_bad++; else n_bad = 0;
-      if (n_bad >= 3) { ok = false; continue; }
+      if (n_bad >= 3) { ok = false; end = 3; continue; }
     }
+    if (trace) { trace[0] = end; trace[1] = done; trace[2] = iterations; }
     return done;
+  }
+  // trace only, over the edges with use(e): chi2 of the cached errors the classification read and of fresh errors at est, the
+  // number of edges whose cached error is not bit-identical to the fresh one, and the classification's rejections
+  template <class Use>
+  void trace_chi2(Use use, int rejected) const {
+    if (!trace) return;
+    double cached = 0, fresh = 0, stale = 0;
+    for (int e = 0; e < m.n_edges(); e++) {
+      if (!use(e)) continue;
+      double f[2];
+      m.error(est, e, f);
+      const double w = m.weight(e);
+      cached += chi2_of(e);
+      fresh += f[0] * (w * f[0]) + f[1] * (w * f[1]);
+      stale += (err[2 * e] != f[0] || err[2 * e + 1] != f[1]) ? 1 : 0;
+    }
+    trace[3] = cached; trace[4] = fresh; trace[5] = stale; trace[6] = rejected;
   }
 };
 
-}  // namespace
 
-extern "C" int orc_pose_optimize(const orc_pose_opt_problem* p, double* Tcw_out, uint8_t* outlier) {
+int pose_optimize(const orc_pose_opt_problem* p, double* Tcw_out, uint8_t* outlier, double* trace) {
   Single<PoseModel> s;
   s.m.p = p;
   const int N = p->n;
@@ -266,6 +296,7 @@ extern "C" int orc_pose_optimize(const orc_pose_opt_problem* p, double* Tcw_out,
   int nBad = 0;
   for (int round = 0; round < 4; round++) {
     s.est = T0;          // vSE3->setEstimate(Converter::toSE3Quat(Frame.mTcw))
+    s.trace = trace ? trace + (size_t)round * TRACE_CALL : nullptr;
     s.optimize(10);      // initializeOptimization(0) = the level-0 edges = s.active
     nBad = 0;
     for (int e = 0; e < N; e++) {
@@ -274,13 +305,14 @@ extern "C" int orc_pose_optimize(const orc_pose_opt_problem* p, double* Tcw_out,
       if (chi2 > 5.991f) { outlier[e] = 1; s.active[e] = 0; nBad++; } else { outlier[e] = 0; s.active[e] = 1; }
       if (round == 2) s.robust[e] = 0;                     // e->setRobustKernel(0)
     }
+    s.trace_chi2([](int) { return true; }, nBad);       // s.err now holds what the classification read, for every edge
     if (N < 10) break;  // optimizer.edges().size() < 10
   }
   se3_store(s.est, Tcw_out);
   return N - nBad;
 }
 
-extern "C" int orc_sim3_optimize(const orc_sim3_opt_problem* p, double* S12_out, uint8_t* inlier) {
+int sim3_optimize(const orc_sim3_opt_problem* p, double* S12_out, uint8_t* inlier, double* trace) {
   Single<Sim3Model> s;
   s.m.p = p;
   const int N = p->n;
@@ -289,22 +321,45 @@ extern "C" int orc_sim3_optimize(const orc_sim3_opt_problem* p, double* S12_out,
   s.est = sim3_load(p->S12);
   std::memcpy(S12_out, p->S12, 8 * sizeof(double));
   std::fill(inlier, inlier + N, 1);
+  s.trace = trace;
   s.optimize(5);
   int nBad = 0;
   for (int i = 0; i < N; i++)
     if (s.chi2_of(2 * i) > (double)p->th2 || s.chi2_of(2 * i + 1) > (double)p->th2) {
       inlier[i] = 0; s.active[2 * i] = 0; s.active[2 * i + 1] = 0; nBad++;  // removeEdge(e12), removeEdge(e21)
     }
+  s.trace_chi2([](int) { return true; }, nBad);
   const int more = nBad > 0 ? 10 : 5;
   if (N - nBad < 10) return 0;  // g2oS12 is left untouched
+  s.trace = trace ? trace + TRACE_CALL : nullptr;
   s.optimize(more);
   int nIn = 0;
   for (int i = 0; i < N; i++) {
     if (!inlier[i]) continue;
     if (s.chi2_of(2 * i) > (double)p->th2 || s.chi2_of(2 * i + 1) > (double)p->th2) inlier[i] = 0; else nIn++;
   }
+  s.trace_chi2([&](int e) { return s.active[e] != 0; }, N - nBad - nIn);  // the pairs that were still edges
   sim3_store(s.est, S12_out);
   return nIn;
+}
+
+}  // namespace
+
+extern "C" int orc_pose_optimize(const orc_pose_opt_problem* p, double* Tcw_out, uint8_t* outlier) {
+  return pose_optimize(p, Tcw_out, outlier, nullptr);
+}
+extern "C" int orc_sim3_optimize(const orc_sim3_opt_problem* p, double* S12_out, uint8_t* inlier) {
+  return sim3_optimize(p, S12_out, inlier, nullptr);
+}
+// the same, recording g2o's Levenberg protocol of every optimize() call: 4 (pose) / 2 (Sim3) calls of TRACE_CALL doubles, NaN where
+// a call or an iteration did not happen.  The trace only observes: the results are those of orc_pose_optimize / orc_sim3_optimize.
+extern "C" int orc_pose_opt_trace(const orc_pose_opt_problem* p, double* Tcw_out, uint8_t* outlier, double* trace) {
+  std::fill(trace, trace + 4 * TRACE_CALL, std::numeric_limits<double>::quiet_NaN());
+  return pose_optimize(p, Tcw_out, outlier, trace);
+}
+extern "C" int orc_sim3_opt_trace(const orc_sim3_opt_problem* p, double* S12_out, uint8_t* inlier, double* trace) {
+  std::fill(trace, trace + 2 * TRACE_CALL, std::numeric_limits<double>::quiet_NaN());
+  return sim3_optimize(p, S12_out, inlier, trace);
 }
 
 // ---- pieces, for the reference pin of the edge types (tests/test_oracle_vs_reference_g2o.py) ------------------------------------
