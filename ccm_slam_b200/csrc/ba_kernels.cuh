@@ -6,21 +6,24 @@
 //   o_kf,o_lm [El]    i32       observation -> keyframe index / local landmark index (landmark order)
 //   o_uv      [El]    float2    undistorted pixel
 //   o_w       [El]    f32       invSigma2; sign bit = "no robust kernel"; 0 = inactive edge (level 1)
-//   W         [18][Ep] f64 SoA  Hpl block per observation (6x3 row-major entry c at W[c*Ep+e]) -> coalesced stores
 //   Z         [El][18] f64 AoS  W * U^-1 with (Hll + lambda I) = U^T U; gathered 144 B rows by the Schur products
+//             (W = Hpl block per observation, 6x3, lives in shared memory only; ccm_ba_debug_build exports it as [18][Ep] SoA)
 //   Hll       [6][Pl]  f64 SoA  upper triangle (00 01 02 11 12 22);  bl [3][Pl]
 //   Hpp       [Kf][36], bp [Kf][6] ; U_val [nub][36] upper Schur blocks ; s_val [nnzb][36] full block-CSR for PCG
+//   units     [nunits+1] i32    landmark-aligned CTA schedule of k_linearize / k_backsub_points (runs of whole landmarks)
 //
 // Kernels (reference loop each one replaces: SURVEY.md §2.2 K1..K7):
-//   k_linearize   K1+K2  residual + Huber + Jacobians + W store + Hll/bl warp-segmented reduction + chi2
+//   k_linearize   K1..K4 residual + Huber + Jacobians + chi2, Hll/bl summed per landmark in the CTA (no atomics), and with lambda
+//                        Z = W U^-1, g = U^-T bl (lambda folded in, no setLambda/restoreDiagonal passes); a Z-only launch after a
+//                        rejected trial
 //   k_pose_pass   K2     Hpp/bp per free pose (CTA per pose, register accumulation, no atomics)
 //   k_residual    K1     robust chi2 of a trial state
-//   k_scale       K3/K4  Z = W U^-1, g = U^-T bl        (lambda folded in here, no setLambda/restoreDiagonal passes)
 //   k_schur       K4     S_ab = sum_l Z_al Z_bl^T over precomputed product lists (register accumulation, no atomics)
 //   k_finalize_S  K4     S = [a==b](Hpp + lambda I) - products, mirrored to full block-CSR
 //   k_block_jacobi K5    6x6 inverses of the diagonal blocks + bschur
 //   k_pcg         K5     persistent cooperative PCG on the reduced camera system
-//   k_update_poses / k_backsub_points  K6+K7  back-substitution, oplus into the trial state, gain-ratio denominator
+//   k_update_poses / k_backsub_points  K6+K7  back-substitution (landmark-aligned, Z rows coalesced), oplus into the trial state,
+//                                             gain-ratio denominator
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -44,85 +47,178 @@ __device__ __forceinline__ Pose load_pose(const double* __restrict__ pose, int k
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// K1+K2: one thread per observation (landmark order).
-//   reads  20 B/obs (kf, lm, uv, w) + gathers (pose 56 B, intr 32 B, point 24 B: cache resident)
-//   writes 144 B/obs (W, SoA, fully coalesced) + 72 B/landmark (Hll, bl) via warp-segmented reduction
-template <int MINB>
-__global__ void __launch_bounds__(TPB, MINB) k_linearize(
-    const int* __restrict__ o_kf, const int* __restrict__ o_lm, const float2* __restrict__ o_uv,
-    const float* __restrict__ o_w, const double* __restrict__ pose, const double* __restrict__ intr,
-    const int* __restrict__ pose_slot, const double* __restrict__ pt, int E, size_t Ep, int Pl, int robust,
-    double delta, double* __restrict__ W, double* __restrict__ Hll, double* __restrict__ bl,
-    double* __restrict__ chi2_partials) {
-  __shared__ double red[TPB / 32];
-  double chi_acc = 0.0;
-  const int lane = threadIdx.x & 31;
-  for (long long base = (long long)blockIdx.x * TPB; base < E; base += (long long)gridDim.x * TPB) {
-    const long long e = base + threadIdx.x;
-    const bool valid = e < E;
-    int lm = -1;
-    double h[9];  // Hll upper (6) + bl (3)
+// Landmark-aligned CTA schedule (k_linearize, k_backsub_points): a unit is a run [units[c], units[c+1]) of whole landmarks, cut
+// once per handle by k_lin_heads + a scan.  A unit of landmarks with <= LIN_SMALL observations each holds <= LIN_TILE observations
+// (its landmarks all start inside one bucket of LIN_BUCKET observations, the last one ends < LIN_SMALL past it); a larger landmark
+// is a unit of its own, walked in chunks of LIN_TILE.  A unit holds <= LIN_TILE landmarks (runs of empty ones are cut too).
+constexpr int LIN_TILE = 128;    // threads of a CTA = observations per chunk
+constexpr int LIN_SMALL = 32;
+constexpr int LIN_BUCKET = LIN_TILE - LIN_SMALL + 1;
+static_assert(LIN_TILE % 32 == 0 && LIN_SMALL < LIN_TILE, "schedule constants");
+
+__global__ void __launch_bounds__(TPB) k_lin_heads(const int* __restrict__ lm_ptr, int Pl, int* __restrict__ head) {
+  const int l = blockIdx.x * TPB + threadIdx.x;
+  if (l >= Pl) return;
+  const int b = lm_ptr[l], n = lm_ptr[l + 1] - b;
+  int h = l % LIN_TILE == 0 || n > LIN_SMALL;
+  if (!h) {
+    const int bprev = lm_ptr[l - 1];
+    h = b / LIN_BUCKET != bprev / LIN_BUCKET || b - bprev > LIN_SMALL;
+  }
+  head[l] = h;
+}
+
+// K1+K2 of one observation for the thread's slot t of the chunk [c0, c1): the 6x3 W row into s_w (row stride 19), and with
+// hsum the 9 point-side terms (Hll upper, bl) into s_h and the robust chi2 into chi.  dbgW (debug export only): W as
+// [18][Ep] SoA.  Returns the observation's landmark (-1 past the chunk).
+__device__ __forceinline__ int lin_obs(int c0, int c1, const int* __restrict__ o_kf, const int* __restrict__ o_lm,
+                                       const float2* __restrict__ o_uv, const float* __restrict__ o_w,
+                                       const double* __restrict__ pose, const double* __restrict__ intr,
+                                       const int* __restrict__ pose_slot, const double* __restrict__ pt, int robust, double delta,
+                                       bool hsum, double* s_w, double* s_h, double& chi, double* __restrict__ dbgW, size_t Ep) {
+  const int t = threadIdx.x;
+  const int e = c0 + t;
+  if (e >= c1) return -1;
+  const int kf = o_kf[e];
+  const int lm = o_lm[e];
+  const float2 uv = o_uv[e];
+  const float wf = o_w[e];
+  const double w = fabs((double)wf);
+  const bool rob = robust && !signbit(wf);
+  const Pose T = load_pose(pose, kf);
+  const double in4[4] = {__ldg(intr + 4 * (size_t)kf), __ldg(intr + 4 * (size_t)kf + 1),
+                         __ldg(intr + 4 * (size_t)kf + 2), __ldg(intr + 4 * (size_t)kf + 3)};
+  const double* X = pt + 3 * (size_t)lm;
+  ObsLin L;
+  linearize_obs(T, in4, X[0], X[1], X[2], (double)uv.x, (double)uv.y, w, L);
+  double rho0 = L.chi2, rho1 = 1.0;
+  if (rob) huber(L.chi2, delta, rho0, rho1);
+  const double wo = rho1 * w;                     // weightedOmega = rho'(chi2) * omega
+  if (hsum) {
+    chi += rho0;
+    const double r0 = -wo * L.ex, r1 = -wo * L.ey;  // omega_r = -omega e * rho'
+    double* h = s_h + t * 9;
+    h[0] = wo * (L.Jl[0] * L.Jl[0] + L.Jl[3] * L.Jl[3]);
+    h[1] = wo * (L.Jl[0] * L.Jl[1] + L.Jl[3] * L.Jl[4]);
+    h[2] = wo * (L.Jl[0] * L.Jl[2] + L.Jl[3] * L.Jl[5]);
+    h[3] = wo * (L.Jl[1] * L.Jl[1] + L.Jl[4] * L.Jl[4]);
+    h[4] = wo * (L.Jl[1] * L.Jl[2] + L.Jl[4] * L.Jl[5]);
+    h[5] = wo * (L.Jl[2] * L.Jl[2] + L.Jl[5] * L.Jl[5]);
+    h[6] = L.Jl[0] * r0 + L.Jl[3] * r1;
+    h[7] = L.Jl[1] * r0 + L.Jl[4] * r1;
+    h[8] = L.Jl[2] * r0 + L.Jl[5] * r1;
+  }
+  // pose-landmark block W = Jp^T (wo I) Jl  (zero when the pose vertex is fixed)
+  const double wz = __ldg(pose_slot + kf) >= 0 ? wo : 0.0;
 #pragma unroll
-    for (int i = 0; i < 9; i++) h[i] = 0.0;
-    if (valid) {
-      const int kf = o_kf[e];
-      lm = o_lm[e];
-      const float2 uv = o_uv[e];
-      const float wf = o_w[e];
-      const double w = fabs((double)wf);
-      const bool rob = robust && !signbit(wf);
-      const Pose T = load_pose(pose, kf);
-      const double in4[4] = {__ldg(intr + 4 * (size_t)kf), __ldg(intr + 4 * (size_t)kf + 1),
-                             __ldg(intr + 4 * (size_t)kf + 2), __ldg(intr + 4 * (size_t)kf + 3)};
-      const double* X = pt + 3 * (size_t)lm;
-      ObsLin L;
-      linearize_obs(T, in4, X[0], X[1], X[2], (double)uv.x, (double)uv.y, w, L);
-      double rho0 = L.chi2, rho1 = 1.0;
-      if (rob) huber(L.chi2, delta, rho0, rho1);
-      chi_acc += rho0;
-      const double wo = rho1 * w;               // weightedOmega = rho'(chi2) * omega
-      const double r0 = -wo * L.ex, r1 = -wo * L.ey;  // omega_r = -omega e * rho'
-      // point block
-      h[0] = wo * (L.Jl[0] * L.Jl[0] + L.Jl[3] * L.Jl[3]);
-      h[1] = wo * (L.Jl[0] * L.Jl[1] + L.Jl[3] * L.Jl[4]);
-      h[2] = wo * (L.Jl[0] * L.Jl[2] + L.Jl[3] * L.Jl[5]);
-      h[3] = wo * (L.Jl[1] * L.Jl[1] + L.Jl[4] * L.Jl[4]);
-      h[4] = wo * (L.Jl[1] * L.Jl[2] + L.Jl[4] * L.Jl[5]);
-      h[5] = wo * (L.Jl[2] * L.Jl[2] + L.Jl[5] * L.Jl[5]);
-      h[6] = L.Jl[0] * r0 + L.Jl[3] * r1;
-      h[7] = L.Jl[1] * r0 + L.Jl[4] * r1;
-      h[8] = L.Jl[2] * r0 + L.Jl[5] * r1;
-      // pose-landmark block W = Jp^T (wo I) Jl  (zero when the pose vertex is fixed)
-      const double wz = __ldg(pose_slot + kf) >= 0 ? wo : 0.0;
+  for (int r = 0; r < 6; r++) {
+    const double a = wz * L.Jp[r], b = wz * L.Jp[6 + r];
 #pragma unroll
-      for (int r = 0; r < 6; r++) {
-        const double a = wz * L.Jp[r], b = wz * L.Jp[6 + r];
-#pragma unroll
-        for (int c = 0; c < 3; c++) W[(size_t)(r * 3 + c) * Ep + e] = a * L.Jl[c] + b * L.Jl[3 + c];
-      }
-    }
-    // segmented (by landmark) warp reduction of the 9 point-side sums; observations of one landmark are contiguous
-#pragma unroll
-    for (int off = 1; off < 32; off <<= 1) {
-      const int lm_o = __shfl_down_sync(0xffffffffu, lm, off);
-      const bool take = (lane + off < 32) && (lm_o == lm);
-#pragma unroll
-      for (int i = 0; i < 9; i++) {
-        const double v = __shfl_down_sync(0xffffffffu, h[i], off);
-        if (take) h[i] += v;
-      }
-    }
-    const int lm_prev = __shfl_up_sync(0xffffffffu, lm, 1);
-    if (lm >= 0 && (lane == 0 || lm_prev != lm)) {
-      // a landmark may straddle warps: red.add into the zeroed accumulators (<= a few partial sums per landmark)
-#pragma unroll
-      for (int i = 0; i < 6; i++) atomicAdd(Hll + (size_t)i * Pl + lm, h[i]);
-#pragma unroll
-      for (int i = 0; i < 3; i++) atomicAdd(bl + (size_t)i * Pl + lm, h[6 + i]);
+    for (int c = 0; c < 3; c++) {
+      const double v = a * L.Jl[c] + b * L.Jl[3 + c];
+      s_w[t * 19 + r * 3 + c] = v;
+      if (dbgW != nullptr) dbgW[(size_t)(r * 3 + c) * Ep + e] = v;
     }
   }
-  const double tot = block_sum(chi_acc, red);
-  if (threadIdx.x == 0) chi2_partials[blockIdx.x] = tot;
+  return lm;
+}
+
+// K1..K4 first half, one CTA per unit of the landmark schedule (grid-stride over the units):
+//   pass 1  per observation: residual, Huber weight, Jacobians, chi2; W row and the Hll / bl terms staged in shared memory;
+//           per landmark a fixed-order sum of its terms (no atomics: deterministic)
+//   factor  per landmark: LIN_H writes Hll / bl; LIN_Z factors Hll + lambda I = U^T U and writes g = U^-T bl
+//   pass 2  (LIN_Z) per observation: Z = W U^-1 in place, written AoS through coalesced rows.  A landmark larger than a chunk
+//           recomputes its W rows here, chunk by chunk.
+// mode is a run-time argument on purpose: a Z-only launch (LIN_Z, recompute at the current state after lambda changed) then runs
+// the same instructions as the fused one and gives bit-identical Z.
+//   reads 20 B/obs + cache-resident gathers ; writes 144 B/obs (Z) + 72 B/landmark (Hll, bl) + 24 B/landmark (g)
+enum { LIN_H = 1, LIN_Z = 2 };
+__global__ void __launch_bounds__(LIN_TILE, 6) k_linearize(
+    const int* __restrict__ units, int nunits, const int* __restrict__ lm_ptr, const int* __restrict__ o_kf,
+    const int* __restrict__ o_lm, const float2* __restrict__ o_uv, const float* __restrict__ o_w, const double* __restrict__ pose,
+    const double* __restrict__ intr, const int* __restrict__ pose_slot, const double* __restrict__ pt, int Pl, int robust,
+    double delta, double lambda, int mode, double* __restrict__ Hll, double* __restrict__ bl, double* __restrict__ gvec,
+    double* __restrict__ Z, double* __restrict__ chi2_partials, double* __restrict__ dbgW, size_t Ep) {
+  __shared__ double s_w[LIN_TILE * 19];   // W rows, then Z rows in place (odd stride: conflict-free row access)
+  __shared__ double s_h[LIN_TILE * 9];    // per observation the 9 terms; then per landmark, in its first slot, their sums, then U
+  __shared__ double red[LIN_TILE / 32];
+  const int t = threadIdx.x;
+  double chi = 0.0;
+  for (int c = blockIdx.x; c < nunits; c += gridDim.x) {
+    const int l0 = units[c], nlm = units[c + 1] - l0;
+    const int ob = lm_ptr[l0], oe = lm_ptr[l0 + nlm];
+    const int nch = oe - ob > LIN_TILE ? (oe - ob + LIN_TILE - 1) / LIN_TILE : 1;   // > 1: the unit is one landmark
+    int slot = 0;        // s_h slot of this thread's landmark
+    double acc = 0.0;    // nch > 1: thread i < 9 carries term i over the chunks
+    for (int k = 0; k < nch; k++) {
+      const int c0 = ob + k * LIN_TILE, c1 = min(oe, c0 + LIN_TILE);
+      const int lm = lin_obs(c0, c1, o_kf, o_lm, o_uv, o_w, pose, intr, pose_slot, pt, robust, delta, true, s_w, s_h, chi, dbgW, Ep);
+      if (nch == 1 && lm >= 0) slot = __ldg(lm_ptr + lm) - ob;
+      __syncthreads();
+      for (int q = t; q < nlm * 9; q += LIN_TILE) {
+        const int j = q / 9, i = q - 9 * j;
+        const int b = max(__ldg(lm_ptr + l0 + j), c0), e = min(__ldg(lm_ptr + l0 + j + 1), c1);
+        double v = 0.0;
+        for (int o = b; o < e; o++) v += s_h[(o - c0) * 9 + i];
+        if (nch == 1) {
+          if (e > b) s_h[(b - c0) * 9 + i] = v;   // column i of this landmark's rows is read by this thread only
+        } else {
+          acc += v;
+          if (k == nch - 1) s_h[i] = acc;
+        }
+      }
+      __syncthreads();
+    }
+    if (t < nlm) {
+      const int l = l0 + t, b = __ldg(lm_ptr + l);
+      const bool empty = __ldg(lm_ptr + l + 1) == b;
+      double* hs = s_h + (nch > 1 ? 0 : (b - ob) * 9);
+      double d[9];
+#pragma unroll
+      for (int i = 0; i < 9; i++) d[i] = empty ? 0.0 : hs[i];
+      if (mode & LIN_H) {
+#pragma unroll
+        for (int i = 0; i < 6; i++) Hll[(size_t)i * Pl + l] = d[i];
+#pragma unroll
+        for (int i = 0; i < 3; i++) bl[(size_t)i * Pl + l] = d[6 + i];
+      }
+      if (mode & LIN_Z) {
+        d[0] += lambda; d[3] += lambda; d[5] += lambda;
+        double u[6], g[3];
+        chol3_upper(d, u);
+        UTinv_times(u, d + 6, g);
+        gvec[3 * (size_t)l] = g[0]; gvec[3 * (size_t)l + 1] = g[1]; gvec[3 * (size_t)l + 2] = g[2];
+        if (!empty)
+#pragma unroll
+          for (int i = 0; i < 6; i++) hs[i] = u[i];
+      }
+    }
+    __syncthreads();
+    if (!(mode & LIN_Z)) continue;
+    for (int k = 0; k < nch; k++) {
+      const int c0 = ob + k * LIN_TILE, c1 = min(oe, c0 + LIN_TILE);
+      if (nch > 1) {
+        double unused = 0.0;
+        lin_obs(c0, c1, o_kf, o_lm, o_uv, o_w, pose, intr, pose_slot, pt, robust, delta, false, s_w, s_h, unused, nullptr, Ep);
+        __syncthreads();
+      }
+      if (c0 + t < c1) {
+        const double* u = s_h + slot * 9;
+#pragma unroll
+        for (int r = 0; r < 6; r++) {
+          double* row = s_w + t * 19 + r * 3;
+          row_times_Uinv(u, row[0], row[1], row[2], row[0], row[1], row[2]);
+        }
+      }
+      __syncthreads();
+      const int n = (c1 - c0) * 18;
+      double* out = Z + (size_t)c0 * 18;
+      for (int i = t; i < n; i += LIN_TILE) out[i] = s_w[(i / 18) * 19 + (i % 18)];
+      __syncthreads();
+    }
+  }
+  const double tot = block_sum(chi, red);
+  if (t == 0) chi2_partials[blockIdx.x] = tot;
 }
 
 // K1 on a (trial) state: robust chi2 only.  20 B/obs read.
@@ -280,45 +376,6 @@ __global__ void __launch_bounds__(1024) k_sum_partials(const double* __restrict_
   for (int i = threadIdx.x; i < n; i += blockDim.x) v += partials[i];
   const double t = block_sum(v, red);
   if (threadIdx.x == 0) out[0] = t;
-}
-
-// ------------------------------------------------------------------------------------------------------------
-// K3/K4 first half: Z = W U^-1 (AoS, staged through shared memory for coalesced rows), g = U^-T bl.
-// reads 144 B/obs (W) + cached Hll ; writes 144 B/obs (Z)
-__global__ void __launch_bounds__(TPB) k_scale(const int* __restrict__ o_lm, const double* __restrict__ W, size_t Ep,
-                                               const double* __restrict__ Hll, const double* __restrict__ bl, int Pl,
-                                               int E, double lambda, double* __restrict__ Z, double* __restrict__ gvec) {
-  __shared__ double tile[TPB * 19];
-  const long long e0 = (long long)blockIdx.x * TPB;
-  const long long e = e0 + threadIdx.x;
-  if (e < E) {
-    const int lm = o_lm[e];
-    double d[6], u[6];
-#pragma unroll
-    for (int i = 0; i < 6; i++) d[i] = __ldg(Hll + (size_t)i * Pl + lm);
-    d[0] += lambda; d[3] += lambda; d[5] += lambda;
-    chol3_upper(d, u);
-#pragma unroll
-    for (int r = 0; r < 6; r++) {
-      const double w0 = W[(size_t)(r * 3) * Ep + e], w1 = W[(size_t)(r * 3 + 1) * Ep + e], w2 = W[(size_t)(r * 3 + 2) * Ep + e];
-      double z0, z1, z2;
-      row_times_Uinv(u, w0, w1, w2, z0, z1, z2);
-      tile[threadIdx.x * 19 + r * 3] = z0;
-      tile[threadIdx.x * 19 + r * 3 + 1] = z1;
-      tile[threadIdx.x * 19 + r * 3 + 2] = z2;
-    }
-    const bool head = (e == 0) || (o_lm[e - 1] != lm);
-    if (head) {
-      const double b3[3] = {__ldg(bl + lm), __ldg(bl + (size_t)Pl + lm), __ldg(bl + 2 * (size_t)Pl + lm)};
-      double g[3];
-      UTinv_times(u, b3, g);
-      gvec[3 * (size_t)lm] = g[0]; gvec[3 * (size_t)lm + 1] = g[1]; gvec[3 * (size_t)lm + 2] = g[2];
-    }
-  }
-  __syncthreads();
-  const long long nvalid = (E - e0 < TPB ? E - e0 : TPB) * 18;
-  double* out = Z + e0 * 18;
-  for (int i = threadIdx.x; i < nvalid; i += TPB) out[i] = tile[(i / 18) * 19 + (i % 18)];
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -944,48 +1001,72 @@ __global__ void __launch_bounds__(TPB) k_update_poses(const double* __restrict__
   if (threadIdx.x == 0) scale_partials[blockIdx.x] = t;
 }
 
-// K6+K7 (landmarks): xl = U^-1 (g - sum_o Z_o^T xp), trial point = point + xl, partial of sum xl (lambda xl + bl)
-__global__ void __launch_bounds__(TPB) k_backsub_points(const int* __restrict__ lm_ptr, const int* __restrict__ o_kf,
-                                                        const int* __restrict__ pose_slot, const double* __restrict__ Z,
-                                                        const double* __restrict__ Hll, const double* __restrict__ bl,
-                                                        const double* __restrict__ x, const double* __restrict__ pt,
-                                                        int Pl, double lambda, double* __restrict__ pt_trial,
-                                                        double* __restrict__ dx_out, double* __restrict__ scale_partials) {
-  __shared__ double red[TPB / 32];
+// K6+K7 (landmarks): xl = U^-1 (g - sum_o Z_o^T xp), trial point = point + xl, partial of sum xl (lambda xl + bl).
+// One CTA per unit of the landmark schedule (grid-stride): one thread per observation forms Z_o^T x_kf(o) from its row, a
+// fixed-order sum per landmark follows, and one thread per landmark solves and writes.
+//   reads 148 B/obs (Z, o_kf) + 96 B/landmark (Hll, bl, point) ; writes 24 B/landmark (+ 24 with dx_out)
+__global__ void __launch_bounds__(LIN_TILE) k_backsub_points(const int* __restrict__ units, int nunits, const int* __restrict__ lm_ptr,
+                                                             const int* __restrict__ o_kf, const int* __restrict__ pose_slot,
+                                                             const double* __restrict__ Z, const double* __restrict__ Hll,
+                                                             const double* __restrict__ bl, const double* __restrict__ x,
+                                                             const double* __restrict__ pt, int Pl, double lambda,
+                                                             double* __restrict__ pt_trial, double* __restrict__ dx_out,
+                                                             double* __restrict__ scale_partials) {
+  __shared__ double s_t[LIN_TILE * 3];
+  __shared__ double red[LIN_TILE / 32];
+  const int t = threadIdx.x;
   double acc = 0.0;
-  for (int l = blockIdx.x * TPB + threadIdx.x; l < Pl; l += gridDim.x * TPB) {
-    double d[6], u[6], b3[3], g[3], t[3] = {0, 0, 0}, xl[3];
+  for (int c = blockIdx.x; c < nunits; c += gridDim.x) {
+    const int l0 = units[c], nlm = units[c + 1] - l0;
+    const int ob = lm_ptr[l0], oe = lm_ptr[l0 + nlm];
+    const int nch = oe - ob > LIN_TILE ? (oe - ob + LIN_TILE - 1) / LIN_TILE : 1;   // > 1: the unit is one landmark (thread 0)
+    double tl[3] = {0.0, 0.0, 0.0};
+    for (int k = 0; k < nch; k++) {
+      const int c0 = ob + k * LIN_TILE, c1 = min(oe, c0 + LIN_TILE);
+      double v0 = 0.0, v1 = 0.0, v2 = 0.0;
+      if (c0 + t < c1) {
+        const int s = __ldg(pose_slot + o_kf[c0 + t]);
+        if (s >= 0) {   // the warp's rows are contiguous: every byte of the lines it touches is used
+          const double2* z2 = reinterpret_cast<const double2*>(Z + (size_t)(c0 + t) * 18);
+          double z[18];
 #pragma unroll
-    for (int i = 0; i < 6; i++) d[i] = Hll[(size_t)i * Pl + l];
-    d[0] += lambda; d[3] += lambda; d[5] += lambda;
-    chol3_upper(d, u);
-    b3[0] = bl[l]; b3[1] = bl[(size_t)Pl + l]; b3[2] = bl[2 * (size_t)Pl + l];
-    UTinv_times(u, b3, g);
-    const int beg = lm_ptr[l], end = lm_ptr[l + 1];
-    for (int o = beg; o < end; o++) {
-      const int s = __ldg(pose_slot + o_kf[o]);
-      if (s < 0) continue;
-      const double2* z2 = reinterpret_cast<const double2*>(Z + (size_t)o * 18);
-      double z[18];
+          for (int i = 0; i < 9; i++) { const double2 v = z2[i]; z[2 * i] = v.x; z[2 * i + 1] = v.y; }
 #pragma unroll
-      for (int i = 0; i < 9; i++) { const double2 v = z2[i]; z[2 * i] = v.x; z[2 * i + 1] = v.y; }
-#pragma unroll
-      for (int r = 0; r < 6; r++) {
-        const double xr = __ldg(x + (size_t)s * 6 + r);
-        t[0] += z[r * 3] * xr; t[1] += z[r * 3 + 1] * xr; t[2] += z[r * 3 + 2] * xr;
+          for (int r = 0; r < 6; r++) {
+            const double xr = __ldg(x + (size_t)s * 6 + r);
+            v0 += z[r * 3] * xr; v1 += z[r * 3 + 1] * xr; v2 += z[r * 3 + 2] * xr;
+          }
+        }
       }
-    }
-    const double gm[3] = {g[0] - t[0], g[1] - t[1], g[2] - t[2]};
-    Uinv_times(u, gm, xl);
+      s_t[t * 3] = v0; s_t[t * 3 + 1] = v1; s_t[t * 3 + 2] = v2;
+      __syncthreads();
+      if (t < nlm) {
+        const int l = l0 + t;
+        const int b = max(__ldg(lm_ptr + l), c0), e = min(__ldg(lm_ptr + l + 1), c1);
+        for (int o = b; o < e; o++) { tl[0] += s_t[(o - c0) * 3]; tl[1] += s_t[(o - c0) * 3 + 1]; tl[2] += s_t[(o - c0) * 3 + 2]; }
+        if (k == nch - 1) {
+          double d[6], u[6], b3[3], g[3], xl[3];
 #pragma unroll
-    for (int c = 0; c < 3; c++) {
-      pt_trial[3 * (size_t)l + c] = pt[3 * (size_t)l + c] + xl[c];
-      acc += xl[c] * (lambda * xl[c] + b3[c]);
-      if (dx_out) dx_out[3 * (size_t)l + c] = xl[c];
+          for (int i = 0; i < 6; i++) d[i] = Hll[(size_t)i * Pl + l];
+          d[0] += lambda; d[3] += lambda; d[5] += lambda;
+          chol3_upper(d, u);
+          b3[0] = bl[l]; b3[1] = bl[(size_t)Pl + l]; b3[2] = bl[2 * (size_t)Pl + l];
+          UTinv_times(u, b3, g);
+          const double gm[3] = {g[0] - tl[0], g[1] - tl[1], g[2] - tl[2]};
+          Uinv_times(u, gm, xl);
+#pragma unroll
+          for (int cc = 0; cc < 3; cc++) {
+            pt_trial[3 * (size_t)l + cc] = pt[3 * (size_t)l + cc] + xl[cc];
+            acc += xl[cc] * (lambda * xl[cc] + b3[cc]);
+            if (dx_out) dx_out[3 * (size_t)l + cc] = xl[cc];
+          }
+        }
+      }
+      __syncthreads();
     }
   }
   const double tt = block_sum(acc, red);
-  if (threadIdx.x == 0) scale_partials[blockIdx.x] = tt;
+  if (t == 0) scale_partials[blockIdx.x] = tt;
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -1138,7 +1219,8 @@ __global__ void __launch_bounds__(TPB) k_tile_heads(const unsigned long long* __
   if (i >= nub) return;
   head[i] = (i == 0 || (keys[i] >> 8) != (keys[i - 1] >> 8)) ? 1 : 0;
 }
-// tile_ptr[t] = first sorted position of tile t (rank = inclusive scan of the heads), tile_ptr[ntiles] = nub
+// tile_ptr[t] = first sorted position of tile t (rank = inclusive scan of the heads), tile_ptr[ntiles] = nub.  Also cuts the
+// landmark schedule of k_linearize (heads from k_lin_heads, n = Pl).
 __global__ void __launch_bounds__(TPB) k_tile_ptr(const int* __restrict__ head, const int* __restrict__ rank, int nub,
                                                   int* __restrict__ tile_ptr) {
   const int i = blockIdx.x * TPB + threadIdx.x;

@@ -68,7 +68,10 @@ struct ccm_ba_handle {
   DevBuf<float> o_w, o_w_raw;
   DevBuf<uint8_t> d_flags;
   // linear system
-  DevBuf<double> W, Z, HllBl, gvec;       // HllBl = [Hll 6*Pl | bl 3*Pl]
+  DevBuf<double> Z, HllBl, gvec;          // HllBl = [Hll 6*Pl | bl 3*Pl]
+  DevBuf<double> W;                       // ccm_ba_debug_build only: allocated on its first call
+  DevBuf<int> units;                      // landmark-aligned CTA schedule of k_linearize / k_backsub_points
+  int nunits = 0, lin_grid = 1, bs_grid = 1;
   DevBuf<double> Hbuf;                    // [Hpp Kf*36 | bp Kf*6 | chi2_cur | maxdiag-bits]
   DevBuf<double> Ubuf;                    // [U_val nub*36 | bneg Kf*6]
   DevBuf<double> s_val, Minv, bschur;
@@ -183,17 +186,19 @@ void collect_spans(ccm_ba_handle* h) {  // call after a stream synchronize
   h->ev_used = 0;
 }
 
-void launch_linearize(ccm_ba_handle* h, int g, int robust, double delta) {
-  // 64 registers / 4 CTAs per SM by default (48 B of L1-resident spill, faster on cfg5 than 80 or 128 registers);
-  // CCM_LIN_MINB=2|3 selects the other builds
-  static const int minb = env_int("CCM_LIN_MINB", 4);
-  cudaStream_t s = h->stream;
-#define CCM_LIN_ARGS h->o_kf.p, h->o_lm.p, h->o_uv.p, h->o_w.p, h->pose_cur, h->intr.p, h->pose_slot.p, h->pt_cur, h->El, h->Ep, \
-                     h->Pl, robust, delta, h->W.p, h->Hll(), h->bl(), h->partials.p
-  if (minb == 2) k_linearize<2><<<g, TPB, 0, s>>>(CCM_LIN_ARGS);
-  else if (minb == 3) k_linearize<3><<<g, TPB, 0, s>>>(CCM_LIN_ARGS);
-  else k_linearize<4><<<g, TPB, 0, s>>>(CCM_LIN_ARGS);
-#undef CCM_LIN_ARGS
+// mode: LIN_H (Hll, bl, chi2 partials) | LIN_Z (g and Z at damping lambda); dbgW: W export of ccm_ba_debug_build
+void launch_linearize(ccm_ba_handle* h, int robust, double delta, int mode, double lambda, double* dbgW = nullptr) {
+  k_linearize<<<h->lin_grid, LIN_TILE, 0, h->stream>>>(h->units.p, h->nunits, h->lm_ptr.p, h->o_kf.p, h->o_lm.p, h->o_uv.p, h->o_w.p,
+                                                      h->pose_cur, h->intr.p, h->pose_slot.p, h->pt_cur, h->Pl, robust, delta, lambda,
+                                                      mode, h->Hll(), h->bl(), h->gvec.p, h->Z.p, h->partials.p, dbgW, h->Ep);
+  CCM_LAUNCHED();
+}
+
+void launch_backsub(ccm_ba_handle* h, double lambda, double* dx_points) {
+  k_backsub_points<<<h->bs_grid, LIN_TILE, 0, h->stream>>>(h->units.p, h->nunits, h->lm_ptr.p, h->o_kf.p, h->pose_slot.p, h->Z.p,
+                                                           h->Hll(), h->bl(), h->x.p, h->pt_cur, h->Pl, lambda, h->pt_trial, dx_points,
+                                                           h->partials.p);
+  CCM_LAUNCHED();
 }
 
 void pack_pose_obs(ccm_ba_handle* h) {
@@ -209,16 +214,14 @@ void sum_partials_to(ccm_ba_handle* h, int n, double* out) {
 }
 
 // ---- kernels wrapped as steps --------------------------------------------------------------------------------
-void step_linearize(ccm_ba_handle* h, int robust, double delta) {
+// linearisation at the current estimate: Hll / bl / chi2 and the pose pass; with LIN_Z in mode also g and Z at lambda
+void step_linearize(ccm_ba_handle* h, int robust, double delta, int mode, double lambda, double* dbgW = nullptr) {
   cudaStream_t s = h->stream;
-  CCM_CUDA(cudaMemsetAsync(h->HllBl.p, 0, h->HllBl.bytes(), s));
-  const int g = grid_stride(h->El);
   {
     KernelSpan sp(h, CCM_BA_K_LINEARIZE);
-    launch_linearize(h, g, robust, delta);
-    CCM_LAUNCHED();
+    launch_linearize(h, robust, delta, LIN_H | mode, lambda, dbgW);
   }
-  sum_partials_to(h, g, h->chi2_cur_dev());
+  sum_partials_to(h, h->lin_grid, h->chi2_cur_dev());
   if (h->Kf > 0) {
     KernelSpan sp(h, CCM_BA_K_POSE_PASS);
     k_pose_pass<<<h->Kf, 128, 0, s>>>(h->kobs.p, h->kobs_ptr.p, h->slot_pose.p, h->pose_cur, h->intr.p, h->pt_cur, robust, delta,
@@ -249,12 +252,11 @@ double read_chi2_cur(ccm_ba_handle* h) {
   return h->h_scal[8];
 }
 
-void step_scale(ccm_ba_handle* h, double lambda) {
-  if (h->El == 0) return;
-  KernelSpan sp(h, CCM_BA_K_SCALE);
-  k_scale<<<div_up(h->El, TPB), TPB, 0, h->stream>>>(h->o_lm.p, h->W.p, h->Ep, h->Hll(), h->bl(), h->Pl, h->El, lambda,
-                                                     h->Z.p, h->gvec.p);
-  CCM_LAUNCHED();
+// g and Z at a new lambda on the unchanged estimate (the first iteration's damping, a rejected trial): the linearisation recomputed,
+// nothing but g and Z written
+void step_z(ccm_ba_handle* h, int robust, double delta, double lambda) {
+  KernelSpan sp(h, CCM_BA_K_LINEARIZE);
+  launch_linearize(h, robust, delta, LIN_Z, lambda);
 }
 
 // CCM_SCHUR selects the Schur-product kernel: "mma" (default: one f64 mma.sync per product, k_schur_mma) or "gather"
@@ -575,11 +577,8 @@ void step_update_and_residual(ccm_ba_handle* h, double lambda, int robust, doubl
   k_update_poses<<<g1, TPB, 0, s>>>(h->pose_cur, h->pose_slot.p, h->x.p, h->bp(), h->K, lambda, h->pose_trial, h->partials.p);
   CCM_LAUNCHED();
   sum_partials_to(h, g1, h->scal.p + 2);
-  const int g2 = grid_stride(h->Pl);
-  k_backsub_points<<<g2, TPB, 0, s>>>(h->lm_ptr.p, h->o_kf.p, h->pose_slot.p, h->Z.p, h->Hll(), h->bl(), h->x.p, h->pt_cur,
-                                      h->Pl, lambda, h->pt_trial, dx_points, h->partials.p);
-  CCM_LAUNCHED();
-  sum_partials_to(h, g2, h->scal.p + 1);
+  launch_backsub(h, lambda, dx_points);
+  sum_partials_to(h, h->bs_grid, h->scal.p + 1);
   if (h->profile) { size_t ev1 = ev_record(h); h->spans.push_back({CCM_BA_K_BACKSUB, ev0, ev1}); ev0 = ev1; }
   const int g3 = grid_stride(h->El);
   k_residual<<<g3, TPB, 0, s>>>(h->o_kf.p, h->o_lm.p, h->o_uv.p, h->o_w.p, h->pose_trial, h->intr.p, h->pt_trial, h->El,
@@ -1037,8 +1036,34 @@ void build(ccm_ba_handle* h, const ccm_ba_problem* p) {
   }
 
   lap("pose observation stream");
+  // ---- landmark-aligned CTA schedule: unit heads (ba_kernels.cuh), numbered by an inclusive scan, cut where a head starts
+  h->nunits = 0;
+  if (Pl > 0) {
+    DevBuf<int> head, rank;
+    head.alloc(Pl); rank.alloc(Pl);
+    k_lin_heads<<<div_up(Pl, TPB), TPB, 0, s>>>(h->lm_ptr.p, Pl, head.p);
+    CCM_LAUNCHED();
+    size_t tb = 0;
+    CCM_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tb, head.p, rank.p, Pl, s));
+    DevBuf<unsigned char> tmp; tmp.alloc(tb + 16);
+    CCM_CUDA(cub::DeviceScan::InclusiveSum(tmp.p, tb, head.p, rank.p, Pl, s));
+    h->units.alloc((size_t)Pl + 1);
+    k_tile_ptr<<<div_up(Pl, TPB), TPB, 0, s>>>(head.p, rank.p, Pl, h->units.p);   // units[rank - 1] = head, units[nunits] = Pl
+    CCM_LAUNCHED();
+    CCM_CUDA(cudaMemcpyAsync(&h->nunits, rank.p + (Pl - 1), sizeof(int), cudaMemcpyDeviceToHost, s));
+    CCM_CUDA(cudaStreamSynchronize(s));   // nunits sizes the grids; the temporaries die here
+  } else {
+    h->units.alloc_zero(1, s);
+  }
+  {
+    int per_sm_lin = 0, per_sm_bs = 0;
+    CCM_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_lin, (const void*)k_linearize, LIN_TILE, 0));
+    CCM_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_bs, (const void*)k_backsub_points, LIN_TILE, 0));
+    h->lin_grid = std::max(1, std::min(h->nunits, sm_count() * std::max(per_sm_lin, 1)));
+    h->bs_grid = std::max(1, std::min(h->nunits, sm_count() * std::max(per_sm_bs, 1)));
+  }
   // ---- linear-system storage
-  h->W.alloc(std::max(h->Ep * 18, (size_t)1)); h->Z.alloc(std::max((size_t)El * 18, (size_t)2));
+  h->Z.alloc(std::max((size_t)El * 18, (size_t)2));
   h->HllBl.alloc(std::max((size_t)Pl * 9, (size_t)1)); h->gvec.alloc(std::max((size_t)Pl * 3, (size_t)1));
   h->Hbuf.alloc_zero((size_t)Kf * 42 + 2, s);
   h->Ubuf.alloc_zero((size_t)nub * 36 + (size_t)Kf * 6 + 1, s);
@@ -1075,7 +1100,7 @@ void build(ccm_ba_handle* h, const ccm_ba_problem* p) {
     h->pcg_Ac.alloc(std::max(2 * nC * nC, (size_t)1)); h->pcg_rc.alloc(std::max(2 * nC, (size_t)1)); h->pcg_yc.alloc(std::max(nC, (size_t)1));
   }
   setup_pcg2(h, h_rowptr);
-  h->partials.alloc((size_t)sm_count() * 8 + 8);
+  h->partials.alloc((size_t)std::max({sm_count() * 8 + 8, h->lin_grid, h->bs_grid}));
   h->scal.alloc_zero(16, s);
   h->rep_chi2.alloc(std::max(El, 1)); h->rep_depth.alloc(std::max(El, 1));
 
@@ -1086,7 +1111,7 @@ void build(ccm_ba_handle* h, const ccm_ba_problem* p) {
   if (Pl) CCM_CUDA(cudaMemcpyAsync(h->pt_trial, h->pt0.p, sizeof(double) * 3 * Pl, cudaMemcpyDeviceToDevice, s));
   h->pose_eval = h->pose_cur; h->pt_eval = h->pt_cur;
   CCM_CUDA(cudaStreamSynchronize(s));
-  h->device_bytes = (int64_t)(h->W.bytes() + h->Z.bytes() + h->prod.bytes() + h->g_ent.bytes() + h->s_val.bytes() + h->Ubuf.bytes() +
+  h->device_bytes = (int64_t)(h->Z.bytes() +h->prod.bytes() + h->g_ent.bytes() + h->s_val.bytes() + h->Ubuf.bytes() +
                               h->bitmap.bytes() + h->word_prefix.bytes() + h->HllBl.bytes() + h->o_kf.bytes() * 2 +
                               h->o_uv.bytes() + h->o_w.bytes() * 2 + h->ptA.bytes() * 3);
   lap("storage + initial state");
@@ -1176,7 +1201,9 @@ void optimize(ccm_ba_handle* h, const ccm_ba_options* o, ccm_ba_result* r) {
   int nBad = 0;
   bool ok = true;
   for (int it = 0; h->Kf > 0 && h->E > 0 && it < o->iterations && !terminate() && ok; it++) {
-    step_linearize(h, robust, delta);
+    // from the second iteration on lambda is known before the linearisation, which then forms Z as well; the first iteration takes
+    // lambda from the diagonal it has just built and forms Z in a second, Z-only pass
+    step_linearize(h, robust, delta, it == 0 ? 0 : LIN_Z, lambda);
     double currentChi;
     if (it == 0) {
       const double maxdiag = step_max_diag(h);
@@ -1188,6 +1215,7 @@ void optimize(ccm_ba_handle* h, const ccm_ba_options* o, ccm_ba_result* r) {
       lambda = o->lambda_init > 0 ? o->lambda_init : 1e-5 * maxdiag;
       ni = 2; nBad = 0;
       r->chi2_initial = currentChi;
+      step_z(h, robust, delta, lambda);
     } else {
       currentChi = read_chi2_cur(h);
     }
@@ -1197,7 +1225,7 @@ void optimize(ccm_ba_handle* h, const ccm_ba_options* o, ccm_ba_result* r) {
     double last_relres = 0;
     do {
       lambda_used = lambda;
-      step_scale(h, lambda);
+      if (qmax > 0) step_z(h, robust, delta, lambda);   // the trial before was rejected: same estimate, larger lambda
       step_schur(h);
       step_finalize(h, lambda);
       step_pcg(h, pcg_tol, pcg_max);
@@ -1399,7 +1427,8 @@ extern "C" int ccm_ba_debug_build(ccm_ba_handle* h, int robust, double huber_del
     CCM_REQUIRE(h->nranks == 1, "debug entry points are single-rank");
     CCM_CUDA(cudaSetDevice(h->device));
     cudaStream_t s = h->stream;
-    step_linearize(h, robust, huber_delta);
+    if (h->W.n < h->Ep * 18) h->W.alloc(std::max(h->Ep * 18, (size_t)1));   // W exists for this export only
+    step_linearize(h, robust, huber_delta, 0, 0.0, h->W.p);
     const int K = h->K, Kf = h->Kf, Pl = h->Pl, El = h->El;
     std::vector<double> hH((size_t)Kf * 42 + 1), hL((size_t)Pl * 9), hW(h->Ep * 18);
     h->Hbuf.download(hH.data(), hH.size(), s); h->HllBl.download(hL.data(), hL.size(), s); h->W.download(hW.data(), hW.size(), s);
@@ -1431,8 +1460,7 @@ extern "C" int ccm_ba_debug_schur(ccm_ba_handle* h, int robust, double huber_del
     CCM_REQUIRE(h->nranks == 1, "debug entry points are single-rank");
     CCM_CUDA(cudaSetDevice(h->device));
     cudaStream_t s = h->stream;
-    step_linearize(h, robust, huber_delta);
-    step_scale(h, lambda);
+    step_linearize(h, robust, huber_delta, LIN_Z, lambda);
     step_schur(h);
     step_finalize(h, lambda);
     step_pcg(h, 1e-13, 5000);
@@ -1542,8 +1570,7 @@ extern "C" int ccm_ba_time_kernel(ccm_ba_handle* h, int which, int reps, double 
     CCM_CUDA(cudaSetDevice(h->device));
     cudaStream_t s = h->stream;
     // make sure every input of the timed kernel exists
-    step_linearize(h, 1, huber_delta);
-    step_scale(h, lambda);
+    step_linearize(h, 1, huber_delta, LIN_Z, lambda);
     step_schur(h);
     step_finalize(h, lambda);
     step_pcg(h, 1e-10, 2000);
@@ -1551,11 +1578,10 @@ extern "C" int ccm_ba_time_kernel(ccm_ba_handle* h, int which, int reps, double 
     CCM_CUDA(cudaEventCreate(&e0)); CCM_CUDA(cudaEventCreate(&e1));
     float total = 0.f;
     for (int i = 0; i < reps; i++) {
-      if (which == 0) CCM_CUDA(cudaMemsetAsync(h->HllBl.p, 0, h->HllBl.bytes(), s));
       CCM_CUDA(cudaEventRecord(e0, s));
       switch (which) {
         case 0:
-          launch_linearize(h, grid_stride(h->El), 1, huber_delta);
+          launch_linearize(h, 1, huber_delta, LIN_H | LIN_Z, lambda);
           break;
         case 1:
           k_pose_pass<<<h->Kf, 128, 0, s>>>(h->kobs.p, h->kobs_ptr.p, h->slot_pose.p, h->pose_cur, h->intr.p, h->pt_cur, 1, huber_delta,
@@ -1566,14 +1592,13 @@ extern "C" int ccm_ba_time_kernel(ccm_ba_handle* h, int which, int reps, double 
                                                         h->pt_cur, h->El, 1, huber_delta, h->partials.p);
           break;
         case 3:
-          k_scale<<<div_up(h->El, TPB), TPB, 0, s>>>(h->o_lm.p, h->W.p, h->Ep, h->Hll(), h->bl(), h->Pl, h->El, lambda, h->Z.p, h->gvec.p);
+          launch_linearize(h, 1, huber_delta, LIN_Z, lambda);
           break;
         case 4:
           launch_schur(h, s);
           break;
         case 5:
-          k_backsub_points<<<grid_stride(h->Pl), TPB, 0, s>>>(h->lm_ptr.p, h->o_kf.p, h->pose_slot.p, h->Z.p, h->Hll(), h->bl(),
-                                                              h->x.p, h->pt_cur, h->Pl, lambda, h->pt_trial, nullptr, h->partials.p);
+          launch_backsub(h, lambda, nullptr);
           break;
         case 6: {
           step_pcg(h, 1e-10, 2000);
@@ -1582,7 +1607,7 @@ extern "C" int ccm_ba_time_kernel(ccm_ba_handle* h, int which, int reps, double 
         default:
           throw Error(CCM_ERR_INVALID, "ccm_ba_time_kernel: unknown kernel id");
       }
-      if (which != 6) CCM_LAUNCHED();
+      if (which == 1 || which == 2 || which == 4) CCM_LAUNCHED();
       CCM_CUDA(cudaEventRecord(e1, s));
       CCM_CUDA(cudaEventSynchronize(e1));
       float ms = 0.f;
@@ -1590,7 +1615,6 @@ extern "C" int ccm_ba_time_kernel(ccm_ba_handle* h, int which, int reps, double 
       total += ms;
     }
     cudaEventDestroy(e0); cudaEventDestroy(e1);
-    if (which == 0) step_linearize(h, 1, huber_delta);  // leave Hll consistent
     *ms_per_launch = total / reps;
   });
 }

@@ -146,9 +146,10 @@ int ccm_ba_get_info(const ccm_ba_handle* h, ccm_ba_info* info);
 
 /* per-kernel CUDA-event accounting over everything ccm_ba_optimize launches while profiling is on (events are
  * recorded on the handle's stream around each kernel / kernel group; two records per span). */
-#define CCM_BA_K_LINEARIZE 0   /* k_linearize: residual + Jacobian + W store + Hll/bl            (per LM iteration) */
+#define CCM_BA_K_LINEARIZE 0   /* k_linearize: residual + Jacobian + Hll/bl + Z = W U^-1         (per LM iteration; Z-only
+                                  launches in the first iteration and after a rejected trial) */
 #define CCM_BA_K_POSE_PASS 1   /* k_pose_pass: Hpp/bp                                            (per LM iteration) */
-#define CCM_BA_K_SCALE 2       /* k_scale: Z = W U^-1                                            (per LM trial) */
+#define CCM_BA_K_SCALE 2       /* no kernel: Z is formed by k_linearize (slot kept, records no launches) */
 #define CCM_BA_K_SCHUR 3       /* k_schur: Schur products                                        (per LM trial) */
 #define CCM_BA_K_ALLREDUCE 4   /* NCCL all-reduce of [S upper | bschur part]                     (per LM trial, N>1) */
 #define CCM_BA_K_FINALIZE 5    /* k_finalize_S + k_block_jacobi                                  (per LM trial) */
@@ -181,7 +182,8 @@ int ccm_ba_debug_paths(ccm_ba_handle* h, int32_t* out /*8*/);
  * -1 = back to the CCM_SCHUR environment variable / built-in default */
 int ccm_ba_debug_set_schur_mode(int mode);
 /* time `reps` launches of one kernel with CUDA events on the handle's stream; returns mean ms per launch.
- * which: 0 linearize (landmark pass), 1 pose pass, 2 residual/chi2, 3 scale (W->Z), 4 schur products, 5 back-substitution */
+ * which: 0 linearize (landmark pass, Hll/bl and Z), 1 pose pass, 2 residual/chi2, 3 Z-only linearize (g and Z at lambda),
+ * 4 schur products, 5 back-substitution */
 int ccm_ba_time_kernel(ccm_ba_handle* h, int which, int reps, double huber_delta, double lambda, double* ms_per_launch);
 
 /* Converter::toSE3Quat / toCvMat restated (cslam/src/Converter.cc:40-72) — host-side helpers for the shim */

@@ -18,7 +18,7 @@ t = time.time(); r = h.optimize(iterations=iters, want_state=False); dt = time.t
 print(f"optimize({iters}): {dt:.3f}s iters={r['iters_done']} trials={r['trials_total']} pcg_total={r['pcg_iters_total']} notconv={r['pcg_not_converged']}")
 print("trace [it lambda chi2 rho trials lambda_after pcg_it relres]"); np.set_printoptions(linewidth=200, precision=4)
 print(r["trace"])
-names = ["linearize", "pose_pass", "residual", "scale(W->Z)", "schur", "backsub", "pcg"]
+names = ["linearize", "pose_pass", "residual", "z_only", "schur", "backsub", "pcg"]
 lam = float(r["trace"][0, 1]) if len(r["trace"]) else 1.0
 for i, n in enumerate(names):
     print(f"  kernel {n:12s}: {h.time_kernel(i, reps=3, lam=lam):9.4f} ms")
