@@ -5,7 +5,6 @@ if the library is missing, or no CUDA device is present, the calls raise.
 """
 from __future__ import annotations
 
-import contextlib
 import ctypes as C
 import os
 
@@ -271,11 +270,11 @@ class BAHandle:
         _chk(lib().ccm_ba_debug_schur_blocks(self._h, _p(rowptr), _p(col), _p(val), _p(bs)))
         return dict(rowptr=rowptr, col=col[:nnzb], val=val[:nnzb], bschur=bs)
 
-    PATH_KEYS = ("schur_mode", "panels_on", "panels", "covered", "pcg_impl", "pcg_block", "pcg_agg", "pcg_nc")
+    PATH_KEYS = ("pcg_impl", "pcg_block", "pcg_agg", "pcg_nc")
 
     def debug_paths(self):
-        """what the handle runs: Schur mode in effect, panels, PCG kernel, CTA size and coarse space"""
-        out = np.zeros(8, np.int32)
+        """the PCG path the handle runs: kernel, CTA size and coarse space"""
+        out = np.zeros(4, np.int32)
         _chk(lib().ccm_ba_debug_paths(self._h, _p(out)))
         return {k: int(v) for k, v in zip(self.PATH_KEYS, out)}
 
@@ -295,17 +294,6 @@ class BAHandle:
         ms = C.c_double()
         _chk(lib().ccm_ba_time_kernel(self._h, which, reps, C.c_double(huber_delta), C.c_double(lam), C.byref(ms)))
         return ms.value
-
-
-@contextlib.contextmanager
-def schur_mode(mode: int):
-    """ccm_ba_debug_set_schur_mode for the duration of a block.  The override is process-global, so it is always put back to -1
-    (the CCM_SCHUR environment variable / built-in default), also when the block raises."""
-    _chk(lib().ccm_ba_debug_set_schur_mode(int(mode)))
-    try:
-        yield
-    finally:
-        _chk(lib().ccm_ba_debug_set_schur_mode(-1))
 
 
 def poses_from_Tcw_f32(T):

@@ -18,7 +18,7 @@
 //                        rejected trial
 //   k_pose_pass   K2     Hpp/bp per free pose (CTA per pose, register accumulation, no atomics)
 //   k_residual    K1     robust chi2 of a trial state
-//   k_schur       K4     S_ab = sum_l Z_al Z_bl^T over precomputed product lists (register accumulation, no atomics)
+//   k_schur_mma   K4     S_ab = sum_l Z_al Z_bl^T over precomputed product lists (register accumulation, no atomics)
 //   k_finalize_S  K4     S = [a==b](Hpp + lambda I) - products, mirrored to full block-CSR
 //   k_block_jacobi K5    6x6 inverses of the diagonal blocks + bschur
 //   k_pcg         K5     persistent cooperative PCG on the reduced camera system
@@ -379,112 +379,35 @@ __global__ void __launch_bounds__(1024) k_sum_partials(const double* __restrict_
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// K4: Schur products.  One warp per upper block u = (a,b): lane = (row r = lane % 6, stream s = lane / 6), 5 streams.
-//   acc[r][c] += sum_k Z_oa[r][k] * Z_ob[c][k]  over the block's product list; diagonal blocks also build
-//   bneg_a = sum_o Z_o g_l(o).  Outputs are written NEGATED (S = Hpp + lambda I - sum).
-__global__ void __launch_bounds__(TPB) k_schur(const uint2* __restrict__ prod, const unsigned* __restrict__ u_prod_ptr,
-                                               const int* __restrict__ u_row, const int* __restrict__ u_col, int nub,
-                                               const double* __restrict__ Z, const int* __restrict__ o_lm,
-                                               const double* __restrict__ gvec, double* __restrict__ U_val,
-                                               double* __restrict__ bneg, const unsigned char* __restrict__ covered = nullptr) {
-  const int warp = (int)(((long long)blockIdx.x * TPB + threadIdx.x) >> 5);
-  if (warp >= nub) return;
-  if (covered != nullptr && covered[warp]) return;  // this block belongs to the panel kernel (schur_panel.cuh)
-  const int lane = threadIdx.x & 31;
-  const int r = lane % 6, s = lane / 6;  // lanes 30,31: s == 5 -> idle stream
-  const unsigned beg = u_prod_ptr[warp], end = u_prod_ptr[warp + 1];
-  const bool diag = u_row[warp] == u_col[warp];
-  double acc[6] = {0, 0, 0, 0, 0, 0};
-  double bacc = 0.0;
-  if (s < 5) {
-    for (unsigned p = beg + s; p < end; p += 5) {
-      const uint2 pr = prod[p];
-      const double* za = Z + (size_t)pr.x * 18 + r * 3;
-      const double a0 = za[0], a1 = za[1], a2 = za[2];
-      const double2* zb = reinterpret_cast<const double2*>(Z + (size_t)pr.y * 18);
-      double b[18];
-#pragma unroll
-      for (int i = 0; i < 9; i++) {
-        const double2 t = zb[i];
-        b[2 * i] = t.x; b[2 * i + 1] = t.y;
-      }
-#pragma unroll
-      for (int c = 0; c < 6; c++) acc[c] += a0 * b[c * 3] + a1 * b[c * 3 + 1] + a2 * b[c * 3 + 2];
-      if (diag) {
-        const double* g = gvec + 3 * (size_t)o_lm[pr.x];
-        bacc += a0 * g[0] + a1 * g[1] + a2 * g[2];
-      }
-    }
-  }
-  // combine the 5 streams: lane r gathers lanes r+6, r+12, r+18, r+24
-#pragma unroll
-  for (int c = 0; c < 6; c++) {
-    double v = acc[c];
-    v += __shfl_sync(0xffffffffu, acc[c], (r + 6) & 31) + __shfl_sync(0xffffffffu, acc[c], (r + 12) & 31) +
-         __shfl_sync(0xffffffffu, acc[c], (r + 18) & 31) + __shfl_sync(0xffffffffu, acc[c], (r + 24) & 31);
-    acc[c] = v;
-  }
-  {
-    double v = bacc;
-    v += __shfl_sync(0xffffffffu, bacc, (r + 6) & 31) + __shfl_sync(0xffffffffu, bacc, (r + 12) & 31) +
-         __shfl_sync(0xffffffffu, bacc, (r + 18) & 31) + __shfl_sync(0xffffffffu, bacc, (r + 24) & 31);
-    bacc = v;
-  }
-  if (lane < 6) {
-#pragma unroll
-    for (int c = 0; c < 6; c++) U_val[(size_t)warp * 36 + r * 6 + c] = -acc[c];
-    if (diag) bneg[(size_t)u_row[warp] * 6 + r] = -bacc;
-  }
-}
-
-// K4, tensor-core form (CCM_SCHUR=mma).  The gather form above spends its time in L1TEX wavefronts: every lane of a
-// stream pulls 21 doubles per product.  Here one product Z_oa (6x3) . Z_ob^T (3x6) is ONE mma.sync.m8n8k4.f64 whose
-// operand fragments are exactly one coalesced 144-byte row each:
+// K4: Schur products, tensor-core form.  One warp per upper block u = (a,b) walks the block's precomputed product list
+// (register accumulation, no atomics):
+//   acc[r][c] += sum_k Z_oa[r][k] * Z_ob[c][k]  over the list; diagonal blocks also build bneg_a = sum_o Z_o g_l(o).
+// Outputs are written NEGATED (S = Hpp + lambda I - sum).  One product Z_oa (6x3) . Z_ob^T (3x6) is ONE
+// mma.sync.m8n8k4.f64 whose operand fragments are exactly one coalesced 144-byte row each:
 //   A (8x4 row-major): lane t holds A[t/4][t%4] = Z_oa[t/4][t%4]        rows 6,7 and column 3 are zero padding
 //   B (4x8 col-major): lane t holds B[t%4][t/4] = Z_ob[t/4][t%4]        -> the same offset (t/4)*3 + t%4 into the row
 //   C (8x8)          : lane t holds C[t/4][2*(t%4)], C[t/4][2*(t%4)+1]  accumulated in place over the product list
-// i.e. 18 lanes x 8 B per operand (2 cache lines), no shuffles, no cross-lane reduction.  Diagonal blocks put g_l into
-// B's column 6, so C[r][6] = sum_o Z_o[r][:] . g_l(o) = bneg comes out of the same instruction.  Two accumulator sets
-// (products alternate) keep two MMA chains in flight; they are added in a fixed order: deterministic per list order.
+// i.e. 18 lanes x 8 B per operand (2 cache lines), no cross-lane reduction.  Diagonal blocks put g_l into B's column 6, so
+// C[r][6] = sum_o Z_o[r][:] . g_l(o) = bneg comes out of the same instruction.  Two accumulator sets (products alternate) keep
+// two MMA chains in flight; they are added in a fixed order: deterministic per list order.
+// The kernel is bound by the L1 data pipe's wavefront rate, so the UNROLL list entries of a batch come in with ONE coalesced load
+// (lane j takes entry j) and reach the other lanes by shuffle, instead of UNROLL broadcast loads.  Off-diagonal blocks request the
+// entries of batch k+1 before the rows of batch k, so the entry -> row dependence costs one memory latency per batch instead of two.
 __device__ __forceinline__ void dmma_884(double& c0, double& c1, double a, double b) {
   asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};"
                : "+d"(c0), "+d"(c1)
                : "d"(a), "d"(b));
 }
 
-// TILED: the CTA takes the upper blocks of one T x T tile of S (tile_ptr / tile_u, built by build_schur_tiles): its warps share
-// the Z rows of T block rows and T block columns, and -- the product lists being sorted by landmark -- meet them at about the same
-// time, so most of the 2 x 144 bytes per product come from L1 instead of L2.
-// VEC: the UNROLL list entries of a batch come in with ONE coalesced load (lane j takes entry j) and reach the other lanes by shuffle,
-// instead of UNROLL broadcast loads: the kernel sits at 65 % of the L1 wavefront rate, and the entry loads are a fifth of its wavefronts.
-// PRED (with VEC): the 14 padding lanes of a fragment do not load at all (predicated off) instead of re-reading element 0 of the row.
-// WIDE (with VEC): a 144-byte row comes in as nine 16-byte loads (lanes 0..8) and reaches its fragment lanes by two 64-bit shuffles,
-// instead of eighteen 8-byte lanes: fewer L1 wavefronts per row, more shuffles.
-// SMB (with VEC, CCM_SCHUR=15): the entries of a batch go from the loading lanes through a per-warp shared-memory slot (double-buffered:
-// one __syncwarp per batch) and come back as broadcast 16-byte loads, two entries each: UNROLL / 2 + 1 shared-memory wavefronts per
-// batch instead of 2 UNROLL shuffles (a shuffle is a wavefront of the same L1 data pipe).  Measured slower than shuffles: the
-// store / barrier / load chain in front of every batch costs more latency than the wavefronts are worth.
-template <int UNROLL, int CTA, bool PIPE = false, bool TILED = false, bool VEC = false, bool PRED = false, bool WIDE = false,
-          bool SMB = false>
-__global__ void __launch_bounds__(CTA) k_schur_mma(const uint2* __restrict__ prod, const unsigned* __restrict__ u_prod_ptr,
-                                                   const int* __restrict__ u_row, const int* __restrict__ u_col, int nub,
-                                                   const double* __restrict__ Z, const int* __restrict__ o_lm,
-                                                   const double* __restrict__ gvec, double* __restrict__ U_val,
-                                                   double* __restrict__ bneg, const int* __restrict__ tile_ptr = nullptr,
-                                                   const int* __restrict__ tile_u = nullptr,
-                                                   const unsigned char* __restrict__ covered = nullptr, int only_diag = 0) {
-  static_assert(UNROLL % 2 == 0, "products alternate between two accumulator sets");
-  int warp;
-  if (TILED) {
-    const int t0 = tile_ptr[blockIdx.x], t1 = tile_ptr[blockIdx.x + 1];
-    const int w = threadIdx.x >> 5;
-    if (w >= t1 - t0) return;  // ragged tile (diagonal, band edge): warp-uniform
-    warp = tile_u[t0 + w];
-  } else {
-    warp = (int)(((long long)blockIdx.x * CTA + threadIdx.x) >> 5);
-    if (warp >= nub) return;  // warp-uniform
-  }
-  if (covered != nullptr && covered[warp]) return;  // this block belongs to the panel kernel (schur_panel.cuh)
+constexpr int SCHUR_CTA = 128;   // threads per CTA of k_schur_mma: 4 upper blocks
+__global__ void __launch_bounds__(SCHUR_CTA) k_schur_mma(const uint2* __restrict__ prod, const unsigned* __restrict__ u_prod_ptr,
+                                                         const int* __restrict__ u_row, const int* __restrict__ u_col, int nub,
+                                                         const double* __restrict__ Z, const int* __restrict__ o_lm,
+                                                         const double* __restrict__ gvec, double* __restrict__ U_val,
+                                                         double* __restrict__ bneg) {
+  constexpr int UNROLL = 8;   // products per batch; even: they alternate between the two accumulator sets
+  const int warp = (int)(((long long)blockIdx.x * SCHUR_CTA + threadIdx.x) >> 5);
+  if (warp >= nub) return;  // warp-uniform
   const int lane = threadIdx.x & 31;
   const int m = lane >> 2, k = lane & 3;
   const bool ld = m < 6 && k < 3;
@@ -495,105 +418,16 @@ __global__ void __launch_bounds__(CTA) k_schur_mma(const uint2* __restrict__ pro
   const unsigned beg = u_prod_ptr[warp], end = u_prod_ptr[warp + 1];
   const int row = u_row[warp];
   const bool diag = row == u_col[warp];
-  if (only_diag && !diag) return;  // the off-diagonal blocks belong to k_schur_rowsync
   double c00 = 0.0, c01 = 0.0, c10 = 0.0, c11 = 0.0;
   unsigned p = beg;
-  __shared__ uint4 s_ent[SMB ? (CTA / 32) * 2 * (UNROLL / 2) : 1];   // [warp][buffer][UNROLL entries of 8 bytes]
-  uint4* const my_ent = s_ent + (SMB ? (threadIdx.x >> 5) * 2 * (UNROLL / 2) : 0);
-  unsigned batch = 0;
-  if (!diag && PIPE && VEC) {
+  if (!diag) {
     uint2 nxv = make_uint2(0u, 0u);
     if (p + UNROLL <= end && lane < UNROLL) nxv = prod[p + lane];
     for (; p + UNROLL <= end; p += UNROLL) {
       uint2 pr[UNROLL];
-      if (SMB) {
-        uint4* slot = my_ent + (batch & 1u) * (UNROLL / 2);
-        batch++;
-        if (lane < UNROLL) reinterpret_cast<uint2*>(slot)[lane] = nxv;
-        __syncwarp();
 #pragma unroll
-        for (int j = 0; j < UNROLL; j += 2) {
-          const uint4 t = slot[j >> 1];
-          pr[j] = make_uint2(t.x, t.y); pr[j + 1] = make_uint2(t.z, t.w);
-        }
-      } else {
-#pragma unroll
-        for (int j = 0; j < UNROLL; j++) { pr[j].x = __shfl_sync(0xffffffffu, nxv.x, j); pr[j].y = __shfl_sync(0xffffffffu, nxv.y, j); }
-      }
+      for (int j = 0; j < UNROLL; j++) { pr[j].x = __shfl_sync(0xffffffffu, nxv.x, j); pr[j].y = __shfl_sync(0xffffffffu, nxv.y, j); }
       if (p + 2 * UNROLL <= end && lane < UNROLL) nxv = prod[p + UNROLL + lane];
-      double a[UNROLL], b[UNROLL];
-#pragma unroll
-      for (int j = 0; j < UNROLL; j++) {
-        if (WIDE) {
-          double2 ra = make_double2(0.0, 0.0), rb = make_double2(0.0, 0.0);
-          if (lane < 9) {
-            ra = reinterpret_cast<const double2*>(Z + (size_t)pr[j].x * zs)[lane];
-            rb = reinterpret_cast<const double2*>(Z + (size_t)pr[j].y * zs)[lane];
-          }
-          const int cl = ld ? m * 3 + k : 0, src = cl >> 1;
-          const double ax = __shfl_sync(0xffffffffu, ra.x, src), ay = __shfl_sync(0xffffffffu, ra.y, src);
-          const double bx = __shfl_sync(0xffffffffu, rb.x, src), by = __shfl_sync(0xffffffffu, rb.y, src);
-          a[j] = (cl & 1) ? ay : ax;
-          b[j] = (cl & 1) ? by : bx;
-        } else if (PRED) {
-          a[j] = 0.0; b[j] = 0.0;
-          if (ld) { a[j] = Z[(size_t)pr[j].x * zs + off]; b[j] = Z[(size_t)pr[j].y * zs + off]; }
-        } else {
-          a[j] = Z[(size_t)pr[j].x * zs + off];
-          b[j] = Z[(size_t)pr[j].y * zs + off];
-        }
-      }
-#pragma unroll
-      for (int j = 0; j < UNROLL; j += 2) {
-        dmma_884(c00, c01, ld ? a[j] : 0.0, ld ? b[j] : 0.0);
-        dmma_884(c10, c11, ld ? a[j + 1] : 0.0, ld ? b[j + 1] : 0.0);
-      }
-    }
-    for (; p < end; p++) {
-      const uint2 pr = prod[p];
-      const double a = Z[(size_t)pr.x * zs + off], b = Z[(size_t)pr.y * zs + off];
-      if ((p - beg) & 1u) dmma_884(c10, c11, ld ? a : 0.0, ld ? b : 0.0);
-      else dmma_884(c00, c01, ld ? a : 0.0, ld ? b : 0.0);
-    }
-  } else if (!diag && PIPE) {
-    // software-pipelined form (faster on cfg5 than the plain one): the product entries of batch k+1 are requested before the rows of batch k,
-    // so the entry -> row dependence costs one memory latency per batch instead of two
-    uint2 nx[UNROLL];
-    if (p + UNROLL <= end) {
-#pragma unroll
-      for (int j = 0; j < UNROLL; j++) nx[j] = prod[p + j];
-    }
-    for (; p + UNROLL <= end; p += UNROLL) {
-      uint2 pr[UNROLL];
-#pragma unroll
-      for (int j = 0; j < UNROLL; j++) pr[j] = nx[j];
-      if (p + 2 * UNROLL <= end) {
-#pragma unroll
-        for (int j = 0; j < UNROLL; j++) nx[j] = prod[p + UNROLL + j];
-      }
-      double a[UNROLL], b[UNROLL];
-#pragma unroll
-      for (int j = 0; j < UNROLL; j++) {
-        a[j] = Z[(size_t)pr[j].x * zs + off];
-        b[j] = Z[(size_t)pr[j].y * zs + off];
-      }
-#pragma unroll
-      for (int j = 0; j < UNROLL; j += 2) {
-        dmma_884(c00, c01, ld ? a[j] : 0.0, ld ? b[j] : 0.0);
-        dmma_884(c10, c11, ld ? a[j + 1] : 0.0, ld ? b[j + 1] : 0.0);
-      }
-    }
-    for (; p < end; p++) {
-      const uint2 pr = prod[p];
-      const double a = Z[(size_t)pr.x * zs + off], b = Z[(size_t)pr.y * zs + off];
-      if ((p - beg) & 1u) dmma_884(c10, c11, ld ? a : 0.0, ld ? b : 0.0);
-      else dmma_884(c00, c01, ld ? a : 0.0, ld ? b : 0.0);
-    }
-  } else if (!diag) {
-    for (; p + UNROLL <= end; p += UNROLL) {
-      uint2 pr[UNROLL];
-#pragma unroll
-      for (int j = 0; j < UNROLL; j++) pr[j] = prod[p + j];  // one address for the whole warp
       double a[UNROLL], b[UNROLL];
 #pragma unroll
       for (int j = 0; j < UNROLL; j++) {
@@ -615,39 +449,26 @@ __global__ void __launch_bounds__(CTA) k_schur_mma(const uint2* __restrict__ pro
   } else {
     // diagonal block (Kf of them): lanes 24..26 carry g_l in column 6 of B, so C[r][6] accumulates bneg
     const bool gl = m == 6 && k < 3;
-    if (VEC) {   // batches of UNROLL products: entries by one coalesced load, then all rows, landmark ids and g_l of the batch in flight together
-      for (; p + UNROLL <= end; p += UNROLL) {
-        unsigned ex = 0u;
-        if (lane < UNROLL) ex = prod[p + lane].x;
-        unsigned e[UNROLL];
-        if (SMB && UNROLL % 4 == 0) {
-          uint4* slot = my_ent + (batch & 1u) * (UNROLL / 2);
-          batch++;
-          if (lane < UNROLL) reinterpret_cast<unsigned*>(slot)[lane] = ex;
-          __syncwarp();
+    // batches of UNROLL products: entries by one coalesced load, then all rows, landmark ids and g_l of the batch in flight together
+    for (; p + UNROLL <= end; p += UNROLL) {
+      unsigned ex = 0u;
+      if (lane < UNROLL) ex = prod[p + lane].x;
+      unsigned e[UNROLL];
 #pragma unroll
-          for (int j = 0; j < UNROLL; j += 4) {
-            const uint4 t = slot[j >> 2];
-            e[j] = t.x; e[j + 1] = t.y; e[j + 2] = t.z; e[j + 3] = t.w;
-          }
-        } else {
+      for (int j = 0; j < UNROLL; j++) e[j] = __shfl_sync(0xffffffffu, ex, j);
+      double a[UNROLL], g[UNROLL];
+      int lm[UNROLL];
 #pragma unroll
-          for (int j = 0; j < UNROLL; j++) e[j] = __shfl_sync(0xffffffffu, ex, j);
-        }
-        double a[UNROLL], g[UNROLL];
-        int lm[UNROLL];
+      for (int j = 0; j < UNROLL; j++) {
+        a[j] = Z[(size_t)e[j] * zs + off];
+        lm[j] = gl ? o_lm[e[j]] : 0;
+      }
 #pragma unroll
-        for (int j = 0; j < UNROLL; j++) {
-          a[j] = Z[(size_t)e[j] * zs + off];
-          lm[j] = gl ? o_lm[e[j]] : 0;
-        }
+      for (int j = 0; j < UNROLL; j++) g[j] = gl ? gvec[3 * (size_t)lm[j] + k] : 0.0;
 #pragma unroll
-        for (int j = 0; j < UNROLL; j++) g[j] = gl ? gvec[3 * (size_t)lm[j] + k] : 0.0;
-#pragma unroll
-        for (int j = 0; j < UNROLL; j += 2) {
-          dmma_884(c00, c01, ld ? a[j] : 0.0, gl ? g[j] : (ld ? a[j] : 0.0));
-          dmma_884(c10, c11, ld ? a[j + 1] : 0.0, gl ? g[j + 1] : (ld ? a[j + 1] : 0.0));
-        }
+      for (int j = 0; j < UNROLL; j += 2) {
+        dmma_884(c00, c01, ld ? a[j] : 0.0, gl ? g[j] : (ld ? a[j] : 0.0));
+        dmma_884(c10, c11, ld ? a[j + 1] : 0.0, gl ? g[j + 1] : (ld ? a[j + 1] : 0.0));
       }
     }
     for (; p < end; p++) {
@@ -666,227 +487,6 @@ __global__ void __launch_bounds__(CTA) k_schur_mma(const uint2* __restrict__ pro
     U_val[(size_t)warp * 36 + m * 6 + 2 * k + 1] = -c01;
   }
   if (diag && m < 6 && k == 3) bneg[(size_t)row * 6 + m] = -c00;  // C[m][6]
-}
-
-// Row-synchronous form (CCM_SCHUR=10): a CTA takes up to RS_W consecutive OFF-DIAGONAL upper blocks of ONE block row a (the schedule
-// rs_first / rs_count is cut at row boundaries) and its warps walk their product lists -- sorted by the observation of a, i.e. by
-// landmark -- chunk by chunk of 2^RS_SHIFT observation indices with a CTA barrier after every chunk.  All warps then need the same
-// rows Z_(l, a) at the same time: they are fetched from L2 once per CTA and served from L1 to the other warps, which the free-running
-// list kernel does not achieve (its warps drift apart).  The diagonal blocks (lists four times as long, and the g_l column) stay with
-// k_schur_mma, launched with only_diag = 1.
-constexpr int RS_W = 8;
-constexpr int RS_SHIFT = 13;
-template <int UNROLL>
-__global__ void __launch_bounds__(32 * RS_W) k_schur_rowsync(const uint2* __restrict__ prod, const unsigned* __restrict__ u_prod_ptr,
-                                                             const int* __restrict__ rs_first, const int* __restrict__ rs_count,
-                                                             const double* __restrict__ Z, double* __restrict__ U_val,
-                                                             const unsigned char* __restrict__ covered = nullptr) {
-  __shared__ unsigned s_cmin, s_cmax;
-  const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int count = rs_count[blockIdx.x];
-  // a block the panel kernel owns (schur_panel.cuh) has an empty list here and must not be overwritten; its warp still takes the barriers
-  const bool active = w < count && !(covered != nullptr && covered[rs_first[blockIdx.x] + w]);
-  const int u = active ? rs_first[blockIdx.x] + w : 0;
-  const int m = lane >> 2, k = lane & 3;
-  const bool ld = m < 6 && k < 3;
-  const int off = ld ? m * 3 + k : 0;
-  unsigned p = 0, end = 0;
-  if (active) { p = u_prod_ptr[u]; end = u_prod_ptr[u + 1]; }
-  if (threadIdx.x == 0) { s_cmin = 0xffffffffu; s_cmax = 0u; }
-  __syncthreads();
-  if (active && lane == 0 && p < end) {
-    atomicMin(&s_cmin, prod[p].x >> RS_SHIFT);
-    atomicMax(&s_cmax, prod[end - 1].x >> RS_SHIFT);
-  }
-  __syncthreads();
-  const unsigned cmin = s_cmin, cmax = s_cmax;
-  double c00 = 0.0, c01 = 0.0, c10 = 0.0, c11 = 0.0;
-  // (the last pass, c = cmax + 1 with no limit, takes what a list too long for the set-up sort left out of order)
-  if (cmin != 0xffffffffu)
-    for (unsigned c = cmin; c <= cmax + 1u; c++) {
-      const unsigned lim = c > cmax ? 0xfffffffeu : c;
-      while (p < end) {
-        uint2 pr[UNROLL];
-        int n_in = 0;
-#pragma unroll
-        for (int j = 0; j < UNROLL; j++) {
-          pr[j] = p + j < end ? prod[p + j] : make_uint2(0xffffffffu, 0u);
-          if (pr[j].x != 0xffffffffu && (pr[j].x >> RS_SHIFT) <= lim) n_in = j + 1;   // sorted: the entries of this chunk are a prefix
-        }
-        if (n_in == 0) break;
-        double a[UNROLL], b[UNROLL];
-#pragma unroll
-        for (int j = 0; j < UNROLL; j++) {
-          const bool in = j < n_in;
-          a[j] = (in && ld) ? Z[(size_t)pr[j].x * 18 + off] : 0.0;
-          b[j] = (in && ld) ? Z[(size_t)pr[j].y * 18 + off] : 0.0;
-        }
-#pragma unroll
-        for (int j = 0; j < UNROLL; j += 2) {
-          dmma_884(c00, c01, a[j], b[j]);
-          dmma_884(c10, c11, a[j + 1], b[j + 1]);
-        }
-        p += n_in;
-      }
-      __syncthreads();
-    }
-  if (!active) return;
-  c00 += c10; c01 += c11;
-  if (ld) {
-    U_val[(size_t)u * 36 + m * 6 + 2 * k] = -c00;
-    U_val[(size_t)u * 36 + m * 6 + 2 * k + 1] = -c01;
-  }
-}
-
-// Grouped form (CCM_SCHUR=16 / 17; measured, NOT the default).  The list kernel is bound by the L1 data pipe: every product costs two
-// row loads of 144 bytes (two lines each: ~3 wavefronts), and a row Z_(l,a) is loaded once for every block (a, b) whose list holds l.
-// Here the off-diagonal upper blocks of a block row are cut into groups of QG consecutive blocks (a, b_1 .. b_QG), one warp per group,
-// and the lists are kept per group: an entry is (observation of a, observation of b_1 | none, .., observation of b_QG | none) for one
-// landmark, so the row of a is loaded ONCE per entry and multiplied into up to QG accumulator sets; an entry with one member costs
-// what a list product costs, so the form never loads more rows than the list kernel.  Diagonal blocks (their lists also feed the pose
-// pass, and they carry the g_l column) stay with k_schur_mma, launched with only_diag = 1.
-// Outcome on cfg5: 95.2 M entries for 190 M products (2.0 products per entry: 25 % fewer row loads), parity green
-// (tests/test_gpu_ba.py under CCM_SCHUR=16 and 17), and about 2x slower per launch than the list kernel: 78-128 registers and sixteen
-// conditional MMAs per batch cost more than the row loads saved.  Kept as a switch.
-constexpr int QG = 4;
-constexpr unsigned Q_NONE = 0xffffffffu;
-__device__ __forceinline__ int csr_pos(const unsigned* __restrict__ bitmap, const int* __restrict__ word_prefix,
-                                       const int* __restrict__ s_rowptr, int words, int a, int b);   // defined with the pattern kernels below
-
-// count (fill == 0) or fill (fill == 1) the grouped lists; one thread per local observation e (pose a, landmark l) walks the other
-// observations of l in list order and keeps ONE open entry: an observation of a later pose joins it if it falls into the same group
-// and its member slot is free, otherwise the entry is closed (a slot of the group's list taken by atomicAdd) and a new one opened.
-// Keyframe-ordered observation lists (the usual case) therefore give the densest entries; any other order only costs sharing.
-__global__ void __launch_bounds__(TPB) k_quad_entries(const int* __restrict__ o_kf, const int* __restrict__ o_lm,
-                                                      const int* __restrict__ lm_ptr, const int* __restrict__ pose_slot,
-                                                      const unsigned* __restrict__ bitmap, const int* __restrict__ word_prefix,
-                                                      const int* __restrict__ s_rowptr, const int* __restrict__ csr_u, int words,
-                                                      int E, int fill, const int* __restrict__ u_diag,
-                                                      const int* __restrict__ g_rowstart, unsigned* __restrict__ counters,
-                                                      const unsigned* __restrict__ g_ptr, unsigned* __restrict__ gent) {
-  const long long e = (long long)blockIdx.x * TPB + threadIdx.x;
-  if (e >= E) return;
-  const int a = pose_slot[o_kf[e]];
-  if (a < 0) return;
-  const int lm = o_lm[e];
-  const int beg = lm_ptr[lm], end = lm_ptr[lm + 1];
-  const int ud = u_diag[a], g0 = g_rowstart[a];
-  int open = -1;
-  unsigned m0 = Q_NONE, m1 = Q_NONE, m2 = Q_NONE, m3 = Q_NONE;
-  auto flush = [&]() {
-    if (open < 0) return;
-    const unsigned slot = atomicAdd(counters + open, 1u);
-    if (fill) {
-      unsigned* d = gent + ((size_t)g_ptr[open] + slot) * (QG + 1);
-      d[0] = (unsigned)e; d[1] = m0; d[2] = m1; d[3] = m2; d[4] = m3;
-    }
-  };
-  for (int o = beg; o < end; o++) {
-    const int b = pose_slot[o_kf[o]];
-    if (b <= a) continue;   // strictly upper blocks only (b < 0: fixed pose)
-    const int j = csr_u[csr_pos(bitmap, word_prefix, s_rowptr, words, a, b)] - ud - 1;
-    const int grp = g0 + (j >> 2), mi = j & 3;
-    const unsigned cur = mi == 0 ? m0 : mi == 1 ? m1 : mi == 2 ? m2 : m3;
-    if (grp != open || cur != Q_NONE) {
-      flush();
-      open = grp; m0 = m1 = m2 = m3 = Q_NONE;
-    }
-    if (mi == 0) m0 = (unsigned)o; else if (mi == 1) m1 = (unsigned)o; else if (mi == 2) m2 = (unsigned)o; else m3 = (unsigned)o;
-  }
-  flush();
-}
-
-// a row element if the member is present, 0 otherwise.  Volatile asm: the compiler would otherwise sink every conditional load into the
-// conditional MMA that consumes it (load, wait, multiply, sixteen times in a row) instead of keeping the batch's loads in flight together.
-__device__ __forceinline__ double ld_row_if(const double* p, unsigned present) {
-  double v;
-  asm volatile("{\n .reg .pred q;\n setp.ne.u32 q, %2, 0;\n mov.f64 %0, 0d0000000000000000;\n @q ld.global.nc.f64 %0, [%1];\n}"
-               : "=d"(v)
-               : "l"(p), "r"(present));
-  return v;
-}
-
-// one warp per group; EB entries per batch: their 5 EB words come in with one coalesced load and reach the lanes by shuffle (SMB:
-// through a double-buffered shared-memory slot and broadcast 16-byte loads), then the EB rows of a and the up to QG EB rows of
-// the b_i are in flight together; a member that is absent (warp-uniform) neither loads nor multiplies.
-template <int EB, int CTA, bool SMB>
-__global__ void __launch_bounds__(CTA) k_schur_quad(const unsigned* __restrict__ gent, const unsigned* __restrict__ g_ptr,
-                                                    const int* __restrict__ g_first, const int* __restrict__ g_count, int ng,
-                                                    const double* __restrict__ Z, double* __restrict__ U_val) {
-  static_assert(EB == 4, "a batch is 20 words: five 16-byte pieces");
-  constexpr int NW = EB * (QG + 1);
-  const int warp = (int)(((long long)blockIdx.x * CTA + threadIdx.x) >> 5);
-  if (warp >= ng) return;  // warp-uniform
-  const int lane = threadIdx.x & 31;
-  const int m = lane >> 2, k = lane & 3;
-  const bool ld = m < 6 && k < 3;
-  const int off = ld ? m * 3 + k : (lane < 16 ? 0 : 12);
-  const unsigned beg = g_ptr[warp], end = g_ptr[warp + 1];
-  __shared__ uint4 s_w[SMB ? (CTA / 32) * 2 * (NW / 4) : 1];
-  uint4* const my_w = s_w + (SMB ? (threadIdx.x >> 5) * 2 * (NW / 4) : 0);
-  double c[QG][2][2];
-#pragma unroll
-  for (int i = 0; i < QG; i++) { c[i][0][0] = c[i][0][1] = c[i][1][0] = c[i][1][1] = 0.0; }
-  unsigned p = beg, batch = 0;
-  unsigned nx = Q_NONE;
-  if (p + EB <= end && lane < NW) nx = gent[(size_t)p * (QG + 1) + lane];
-  for (; p + EB <= end; p += EB) {
-    unsigned w[NW];
-    if (SMB) {
-      uint4* slot = my_w + (batch & 1u) * (NW / 4);
-      batch++;
-      if (lane < NW) reinterpret_cast<unsigned*>(slot)[lane] = nx;
-      __syncwarp();
-#pragma unroll
-      for (int j = 0; j < NW; j += 4) {
-        const uint4 t = slot[j >> 2];
-        w[j] = t.x; w[j + 1] = t.y; w[j + 2] = t.z; w[j + 3] = t.w;
-      }
-    } else {
-#pragma unroll
-      for (int j = 0; j < NW; j++) w[j] = __shfl_sync(0xffffffffu, nx, j);
-    }
-    if (p + 2 * EB <= end && lane < NW) nx = gent[(size_t)(p + EB) * (QG + 1) + lane];
-    double a[EB], b[EB][QG];
-#pragma unroll
-    for (int e = 0; e < EB; e++) {
-      a[e] = Z[(size_t)w[e * (QG + 1)] * 18 + off];
-#pragma unroll
-      for (int i = 0; i < QG; i++) {
-        const unsigned ob = w[e * (QG + 1) + 1 + i];
-        b[e][i] = ld_row_if(Z + (size_t)ob * 18 + off, ob != Q_NONE ? 1u : 0u);
-      }
-    }
-#pragma unroll
-    for (int e = 0; e < EB; e++) {
-#pragma unroll
-      for (int i = 0; i < QG; i++)
-        if (w[e * (QG + 1) + 1 + i] != Q_NONE) dmma_884(c[i][e & 1][0], c[i][e & 1][1], ld ? a[e] : 0.0, ld ? b[e][i] : 0.0);
-    }
-  }
-  for (; p < end; p++) {
-    unsigned t = Q_NONE;
-    if (lane < QG + 1) t = gent[(size_t)p * (QG + 1) + lane];
-    const unsigned oa = __shfl_sync(0xffffffffu, t, 0);
-    const double a = Z[(size_t)oa * 18 + off];
-#pragma unroll
-    for (int i = 0; i < QG; i++) {
-      const unsigned ob = __shfl_sync(0xffffffffu, t, 1 + i);
-      if (ob != Q_NONE) {
-        const double b = Z[(size_t)ob * 18 + off];
-        dmma_884(c[i][0][0], c[i][0][1], ld ? a : 0.0, ld ? b : 0.0);
-      }
-    }
-  }
-  const int u0 = g_first[warp], cnt = g_count[warp];
-  if (ld) {
-#pragma unroll
-    for (int i = 0; i < QG; i++)
-      if (i < cnt) {
-        U_val[(size_t)(u0 + i) * 36 + m * 6 + 2 * k] = -(c[i][0][0] + c[i][1][0]);
-        U_val[(size_t)(u0 + i) * 36 + m * 6 + 2 * k + 1] = -(c[i][0][1] + c[i][1][1]);
-      }
-  }
 }
 
 // S (full block-CSR) from the upper blocks: diagonal gets Hpp + lambda I, lower blocks are transposed copies.
@@ -1168,65 +768,14 @@ __global__ void __launch_bounds__(TPB) k_shift(const int* __restrict__ in, long 
   if (i < n) out[i] = in[i] - off;
 }
 
-// Product lists come out of k_products in the order the atomic slots were handed out.  Sorting every list by (first observation,
-// second observation) = by landmark makes the Schur sums deterministic and lets the warps of a tile walk Z together (k_schur_mma,
-// TILED).  One CTA per list, bitonic network in shared memory; lists beyond the shared buffer (a keyframe with more than 4096
-// observations in one block) keep their order, which only costs locality.
-constexpr int SORT_CAP = 4096;
-__global__ void __launch_bounds__(256) k_sort_products(const unsigned* __restrict__ u_prod_ptr, int nub, uint2* __restrict__ prod) {
-  __shared__ unsigned long long s[SORT_CAP];
-  const int u = blockIdx.x;
-  if (u >= nub) return;
-  const unsigned beg = u_prod_ptr[u], end = u_prod_ptr[u + 1];
-  const int n = (int)(end - beg);
-  if (n <= 1 || n > SORT_CAP) return;
-  int m = 2;
-  while (m < n) m <<= 1;
-  for (int i = threadIdx.x; i < m; i += 256) {
-    unsigned long long v = ~0ull;
-    if (i < n) { const uint2 p = prod[beg + i]; v = ((unsigned long long)p.x << 32) | p.y; }
-    s[i] = v;
-  }
-  __syncthreads();
-  for (int k = 2; k <= m; k <<= 1)
-    for (int j = k >> 1; j > 0; j >>= 1) {
-      for (int i = threadIdx.x; i < m; i += 256) {
-        const int ixj = i ^ j;
-        if (ixj > i) {
-          const unsigned long long a = s[i], b = s[ixj];
-          const bool up = (i & k) == 0;
-          if ((a > b) == up) { s[i] = b; s[ixj] = a; }
-        }
-      }
-      __syncthreads();
-    }
-  for (int i = threadIdx.x; i < n; i += 256) prod[beg + i] = make_uint2((unsigned)(s[i] >> 32), (unsigned)(s[i] & 0xffffffffu));
-}
-
-// tile schedule of the upper blocks: key = (row group, column group | position inside the T x T tile), value = block number
-__global__ void __launch_bounds__(TPB) k_tile_keys(const int* __restrict__ u_row, const int* __restrict__ u_col, int nub, int T,
-                                                   unsigned long long ngroups, unsigned long long* __restrict__ keys,
-                                                   int* __restrict__ vals) {
-  const int u = blockIdx.x * TPB + threadIdx.x;
-  if (u >= nub) return;
-  const int a = u_row[u], b = u_col[u];
-  keys[u] = (((unsigned long long)(a / T) * ngroups + (unsigned long long)(b / T)) << 8) | (unsigned)((a % T) * T + (b % T));
-  vals[u] = u;
-}
-// head[i] = 1 where a new tile starts in the sorted key list
-__global__ void __launch_bounds__(TPB) k_tile_heads(const unsigned long long* __restrict__ keys, int nub, int* __restrict__ head) {
+// Cuts the landmark schedule of k_linearize / k_backsub_points: units[r - 1] = i for every head i (head flags from k_lin_heads,
+// rank = their inclusive scan), units[n] = n.
+__global__ void __launch_bounds__(TPB) k_unit_ptr(const int* __restrict__ head, const int* __restrict__ rank, int n,
+                                                  int* __restrict__ units) {
   const int i = blockIdx.x * TPB + threadIdx.x;
-  if (i >= nub) return;
-  head[i] = (i == 0 || (keys[i] >> 8) != (keys[i - 1] >> 8)) ? 1 : 0;
-}
-// tile_ptr[t] = first sorted position of tile t (rank = inclusive scan of the heads), tile_ptr[ntiles] = nub.  Also cuts the
-// landmark schedule of k_linearize (heads from k_lin_heads, n = Pl).
-__global__ void __launch_bounds__(TPB) k_tile_ptr(const int* __restrict__ head, const int* __restrict__ rank, int nub,
-                                                  int* __restrict__ tile_ptr) {
-  const int i = blockIdx.x * TPB + threadIdx.x;
-  if (i >= nub) return;
-  if (head[i]) tile_ptr[rank[i] - 1] = i;
-  if (i == nub - 1) tile_ptr[rank[i]] = nub;
+  if (i >= n) return;
+  if (head[i]) units[rank[i] - 1] = i;
+  if (i == n - 1) units[rank[i]] = n;
 }
 
 // count (fill == 0) or fill (fill == 1) the product lists of the upper blocks; one thread per local observation
@@ -1235,8 +784,7 @@ __global__ void __launch_bounds__(TPB) k_products(const int* __restrict__ o_kf, 
                                                   const unsigned* __restrict__ bitmap, const int* __restrict__ word_prefix,
                                                   const int* __restrict__ s_rowptr, const int* __restrict__ csr_u, int words,
                                                   int E, int fill, unsigned* __restrict__ counters,
-                                                  const unsigned* __restrict__ u_prod_ptr, uint2* __restrict__ prod,
-                                                  const unsigned char* __restrict__ covered = nullptr) {
+                                                  const unsigned* __restrict__ u_prod_ptr, uint2* __restrict__ prod) {
   const long long e = (long long)blockIdx.x * TPB + threadIdx.x;
   if (e >= E) return;
   const int a = pose_slot[o_kf[e]];
@@ -1247,7 +795,6 @@ __global__ void __launch_bounds__(TPB) k_products(const int* __restrict__ o_kf, 
     const int b = pose_slot[o_kf[o]];
     if (b < a || (b == a && o != (int)e)) continue;
     const int u = csr_u[csr_pos(bitmap, word_prefix, s_rowptr, words, a, b)];
-    if (covered != nullptr && b != a && covered[u]) continue;  // the panel kernel forms this block; diagonal lists also feed the pose pass
     const unsigned slot = atomicAdd(counters + u, 1u);
     if (fill) prod[u_prod_ptr[u] + slot] = make_uint2((unsigned)e, (unsigned)o);
   }

@@ -12,13 +12,11 @@
 #include <limits>
 #include <numeric>
 
-#include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
 #include "ba_kernels.cuh"
 #include "common.cuh"
 #include "pcg2.cuh"
-#include "schur_panel.cuh"
 
 namespace ccm {
 void allreduce_f64(double* buf, size_t count, int op, cudaStream_t s);  // runtime.cu ; op: 0 sum, 2 max
@@ -78,21 +76,6 @@ struct ccm_ba_handle {
   DevBuf<int> s_rowptr, s_col, s_row, s_diag, csr_u, u_row, u_col, u_diag, word_prefix;
   DevBuf<unsigned> bitmap, u_prod_ptr;
   DevBuf<uint2> prod;
-  // landmark-synchronous Schur panels (schur_panel.cuh)
-  bool panel_on = false;
-  int npan = 0;
-  DevBuf<int> o_slot, pose_lmin, pose_lmax, pose_cnt;
-  DevBuf<unsigned char> pan_on, covered;
-  DevBuf<int> rs_first, rs_count;  // row-synchronous Schur schedule (CCM_SCHUR=10): CTAs of <= RS_W off-diagonal blocks of one row
-  int rs_ctas = 0;
-  // grouped Schur lists (CCM_SCHUR=16 / 17, k_schur_quad): groups of QG consecutive off-diagonal upper blocks of one row
-  DevBuf<unsigned> g_ptr, g_ent;   // [ng + 1] first entry of every group; entries of QG + 1 words
-  DevBuf<int> g_first, g_count;    // [ng] first upper block and number of blocks of every group
-  int ng = 0;
-  long long nquad = 0;             // grouped entries (local shard)
-  bool quad_built = false;         // the off-diagonal PAIR lists were not built: only k_schur_quad can form those blocks
-  DevBuf<int> tile_ptr, tile_u;   // T x T tiles of upper blocks: the CTA schedule of the tiled Schur kernel
-  int ntiles = 0, tile_T = 0;
   DevBuf<float4> kobs;            // per free pose: (u, v, signed w, landmark) of its observations, packed
   DevBuf<unsigned> kobs_ptr;
   // pcg
@@ -259,134 +242,16 @@ void step_z(ccm_ba_handle* h, int robust, double delta, double lambda) {
   launch_linearize(h, robust, delta, LIN_Z, lambda);
 }
 
-// CCM_SCHUR selects the Schur-product kernel: "mma" (default: one f64 mma.sync per product, k_schur_mma) or "gather"
-// (5 streams x 6 lanes of f64 FMA, k_schur).  Modes 2..5 are launch-shape variants of the mma form kept for tuning runs.
-std::atomic<int> g_schur_override{-1};  // ccm_ba_debug_set_schur_mode
-int schur_mode() {
-  static const int env_mode = [] {
-    const char* v = getenv("CCM_SCHUR");
-    if (!v) return 11;
-    if (!strcmp(v, "gather") || !strcmp(v, "0")) return 0;
-    if (!strcmp(v, "mma")) return 1;
-    const int m = atoi(v);
-    return (m >= 0 && m <= 17) ? m : 1;
-  }();
-  const int o = g_schur_override.load(std::memory_order_relaxed);
-  return o >= 0 ? o : env_mode;
-}
-
-template <int UNROLL, int CTA>
-void launch_schur_tiled(ccm_ba_handle* h, cudaStream_t s) {
-  k_schur_mma<UNROLL, CTA, true, true><<<h->ntiles, CTA, 0, s>>>(h->prod.p, h->u_prod_ptr.p, h->u_row.p, h->u_col.p, h->nub, h->Z.p, h->o_lm.p,
-                                                                  h->gvec.p, h->U_val(), h->bneg(), h->tile_ptr.p, h->tile_u.p,
-                                                                  h->panel_on ? h->covered.p : nullptr);
-}
-
-template <int UNROLL, int CTA, bool PIPE = false>
-void launch_schur_mma(ccm_ba_handle* h, cudaStream_t s) {
-  k_schur_mma<UNROLL, CTA, PIPE><<<div_up((long long)h->nub * 32, CTA), CTA, 0, s>>>(h->prod.p, h->u_prod_ptr.p, h->u_row.p, h->u_col.p, h->nub,
-                                                                              h->Z.p, h->o_lm.p, h->gvec.p, h->U_val(), h->bneg(), nullptr,
-                                                                              nullptr, h->panel_on ? h->covered.p : nullptr);
-}
-
-void launch_schur_panel(ccm_ba_handle* h, cudaStream_t s) {
-  SchurPanelArgs a;
-  a.Z = h->Z.p; a.o_slot = h->o_slot.p; a.lm_ptr = h->lm_ptr.p; a.gvec = h->gvec.p; a.pose_lmin = h->pose_lmin.p; a.pose_lmax = h->pose_lmax.p;
-  a.pan_on = h->pan_on.p; a.Kf = h->Kf; a.bitmap = h->bitmap.p; a.word_prefix = h->word_prefix.p; a.s_rowptr = h->s_rowptr.p;
-  a.csr_u = h->csr_u.p; a.words = h->words; a.U_val = h->U_val(); a.bneg = h->bneg();
-  k_schur_panel<<<h->npan, SP_THREADS, SP_SMEM, s>>>(a);
-}
-
+// K4: the Schur products, one warp per upper block (k_schur_mma)
 void launch_schur(ccm_ba_handle* h, cudaStream_t s) {
-  if (h->panel_on) {   // the band of every enabled panel in registers, fed by TMA; the list kernel below keeps the rest
-    launch_schur_panel(h, s);
-    CCM_LAUNCHED();
-  }
-  const int mode = schur_mode();
-  CCM_REQUIRE(h->quad_built == (mode == 16 || mode == 17),
-              "the grouped Schur lists (CCM_SCHUR=16/17) are built when the handle is created: set the mode before ccm_ba_create");
-  if (h->quad_built) {   // off-diagonal blocks by groups of one row sharing the row of a, diagonal blocks by the list kernel
-    if (h->ng > 0) {
-      if (mode == 17)
-        k_schur_quad<4, 128, true><<<div_up((long long)h->ng * 32, 128), 128, 0, s>>>(h->g_ent.p, h->g_ptr.p, h->g_first.p, h->g_count.p, h->ng, h->Z.p, h->U_val());
-      else
-        k_schur_quad<4, 128, false><<<div_up((long long)h->ng * 32, 128), 128, 0, s>>>(h->g_ent.p, h->g_ptr.p, h->g_first.p, h->g_count.p, h->ng, h->Z.p, h->U_val());
-    }
-    k_schur_mma<8, 128, true, false, true><<<div_up((long long)h->nub * 32, 128), 128, 0, s>>>(h->prod.p, h->u_prod_ptr.p, h->u_row.p, h->u_col.p, h->nub, h->Z.p,
-                                                                                          h->o_lm.p, h->gvec.p, h->U_val(), h->bneg(), nullptr, nullptr, nullptr, 1);
-    return;
-  }
-  if (mode == 10 && h->rs_ctas > 0) {   // off-diagonal blocks row-synchronously, diagonal blocks by the list kernel
-    k_schur_rowsync<8><<<h->rs_ctas, 32 * RS_W, 0, s>>>(h->prod.p, h->u_prod_ptr.p, h->rs_first.p, h->rs_count.p, h->Z.p, h->U_val(),
-                                                         h->panel_on ? h->covered.p : nullptr);
-    k_schur_mma<8, 128, true><<<div_up((long long)h->nub * 32, 128), 128, 0, s>>>(h->prod.p, h->u_prod_ptr.p, h->u_row.p, h->u_col.p, h->nub, h->Z.p,
-                                                                               h->o_lm.p, h->gvec.p, h->U_val(), h->bneg(), nullptr, nullptr,
-                                                                               h->panel_on ? h->covered.p : nullptr, 1);
-    return;
-  }
-  // Modes 11-14: the list kernel is bound by the L1 data pipe's wavefront rate, with two row loads and ONE BROADCAST ENTRY LOAD per
-  // product.  11 (default): the 8 entries of a batch in one coalesced load + shuffles, diagonal blocks batched the same way.
-  // 12: the same at unroll 16.  13: padding lanes predicated off instead of re-reading an element.  14: rows as nine 16-byte loads
-  // + 64-bit shuffles to the fragment lanes (shuffles in bulk cost more than the wavefronts they save).
-  if (mode >= 11 && mode <= 15) {
-    const unsigned char* cov = h->panel_on ? h->covered.p : nullptr;
-    if (mode == 15)   // entries broadcast through shared memory instead of shuffles (slower than mode 11)
-      k_schur_mma<8, 128, true, false, true, false, false, true><<<div_up((long long)h->nub * 32, 128), 128, 0, s>>>(
-          h->prod.p, h->u_prod_ptr.p, h->u_row.p, h->u_col.p, h->nub, h->Z.p, h->o_lm.p, h->gvec.p, h->U_val(), h->bneg(), nullptr, nullptr, cov);
-    else if (mode == 14)
-      k_schur_mma<8, 128, true, false, true, false, true><<<div_up((long long)h->nub * 32, 128), 128, 0, s>>>(h->prod.p, h->u_prod_ptr.p, h->u_row.p, h->u_col.p,
-                                                                                                    h->nub, h->Z.p, h->o_lm.p, h->gvec.p, h->U_val(), h->bneg(),
-                                                                                                    nullptr, nullptr, cov);
-    else if (mode == 13)
-      k_schur_mma<8, 128, true, false, true, true><<<div_up((long long)h->nub * 32, 128), 128, 0, s>>>(h->prod.p, h->u_prod_ptr.p, h->u_row.p, h->u_col.p, h->nub,
-                                                                                             h->Z.p, h->o_lm.p, h->gvec.p, h->U_val(), h->bneg(), nullptr, nullptr, cov);
-    else if (mode == 11)
-      k_schur_mma<8, 128, true, false, true><<<div_up((long long)h->nub * 32, 128), 128, 0, s>>>(h->prod.p, h->u_prod_ptr.p, h->u_row.p, h->u_col.p, h->nub,
-                                                                                       h->Z.p, h->o_lm.p, h->gvec.p, h->U_val(), h->bneg(), nullptr, nullptr, cov);
-    else
-      k_schur_mma<16, 128, true, false, true><<<div_up((long long)h->nub * 32, 128), 128, 0, s>>>(h->prod.p, h->u_prod_ptr.p, h->u_row.p, h->u_col.p, h->nub,
-                                                                                        h->Z.p, h->o_lm.p, h->gvec.p, h->U_val(), h->bneg(), nullptr, nullptr, cov);
-    return;
-  }
-  if (mode == 9 && h->ntiles > 0) {   // tiled schedules (the tile edge was fixed when the handle was created: CCM_SCHUR_TILE)
-    if (h->tile_T == 4) launch_schur_tiled<8, 512>(h, s);
-    else if (h->tile_T == 3) launch_schur_tiled<8, 288>(h, s);
-    else launch_schur_tiled<8, 128>(h, s);
-    return;
-  }
-  switch (mode) {
-    case 0:
-      k_schur<<<div_up((long long)h->nub * 32, TPB), TPB, 0, s>>>(h->prod.p, h->u_prod_ptr.p, h->u_row.p, h->u_col.p, h->nub, h->Z.p,
-                                                                  h->o_lm.p, h->gvec.p, h->U_val(), h->bneg(),
-                                                                  h->panel_on ? h->covered.p : nullptr);
-      break;
-    // launch shapes of the list kernel for tuning runs (tools/schur_variants.py)
-    case 2: launch_schur_mma<16, 256>(h, s); break;
-    case 3: launch_schur_mma<4, 256>(h, s); break;
-    case 4: launch_schur_mma<8, 256>(h, s); break;
-    case 5: launch_schur_mma<8, 512>(h, s); break;
-    case 6: launch_schur_mma<8, 64>(h, s); break;
-    case 7: launch_schur_mma<16, 128>(h, s); break;
-    case 8: launch_schur_mma<8, 128, true>(h, s); break;   // product entries prefetched one batch ahead
-    case 1: launch_schur_mma<8, 128>(h, s); break;
-    default: launch_schur_mma<8, 128, true>(h, s); break;   // mode 11 (above) is the default
-  }
+  k_schur_mma<<<div_up((long long)h->nub * 32, SCHUR_CTA), SCHUR_CTA, 0, s>>>(h->prod.p, h->u_prod_ptr.p, h->u_row.p, h->u_col.p, h->nub,
+                                                                             h->Z.p, h->o_lm.p, h->gvec.p, h->U_val(), h->bneg());
 }
 
 void step_schur(ccm_ba_handle* h) {
   KernelSpan sp(h, CCM_BA_K_SCHUR);
   launch_schur(h, h->stream);
   CCM_LAUNCHED();
-}
-
-// the CCM_SCHUR mode launch_schur actually runs: 9 without a tile schedule and 10 without a row schedule fall through to the
-// prefetching list kernel, which is mode 8
-int schur_path(const ccm_ba_handle* h) {
-  const int mode = schur_mode();
-  if (h->quad_built) return mode;
-  if (mode == 10) return h->rs_ctas > 0 ? 10 : 8;
-  if (mode == 9) return h->ntiles > 0 ? 9 : 8;
-  return mode;
 }
 
 void step_finalize(ccm_ba_handle* h, double lambda) {
@@ -867,83 +732,13 @@ void build(ccm_ba_handle* h, const ccm_ba_problem* p) {
   const int nub = h->nub;
 
   lap("pattern, upper index");
-  // ---- landmark-synchronous Schur panels (CCM_SCHUR_PANEL=1): which upper blocks the panel kernel owns
-  h->panel_on = env_int("CCM_SCHUR_PANEL", 0) != 0 && El > 0 && nub > 0;
-  if (h->panel_on) {
-    h->npan = div_up(Kf, SP_R);
-    h->o_slot.alloc(El); h->pose_lmin.alloc(Kf); h->pose_lmax.alloc(Kf); h->pose_cnt.alloc_zero(Kf, s);
-    k_fill_int<<<div_up(Kf, TPB), TPB, 0, s>>>(h->pose_lmin.p, Kf, 0x7fffffff);
-    k_fill_int<<<div_up(Kf, TPB), TPB, 0, s>>>(h->pose_lmax.p, Kf, -1);
-    k_pose_lm_range<<<div_up(El, TPB), TPB, 0, s>>>(h->o_kf.p, h->o_lm.p, h->pose_slot.p, El, h->o_slot.p, h->pose_lmin.p, h->pose_lmax.p,
-                                                    h->pose_cnt.p);
-    CCM_LAUNCHED();
-    h->pan_on.alloc(h->npan); h->covered.alloc(nub);
-    k_panel_on<<<div_up(h->npan, TPB), TPB, 0, s>>>(h->pose_lmin.p, h->pose_lmax.p, h->lm_ptr.p, h->pose_cnt.p, Kf, h->npan,
-                                                    env_int("CCM_SCHUR_PANEL_FACTOR", 12), h->pan_on.p);
-    CCM_LAUNCHED();
-    k_covered<<<div_up(nub, TPB), TPB, 0, s>>>(h->u_row.p, h->u_col.p, nub, h->pan_on.p, h->covered.p);
-    CCM_LAUNCHED();
-    CCM_CUDA(cudaFuncSetAttribute((const void*)k_schur_panel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SP_SMEM));
-  }
-  const unsigned char* cov = h->panel_on ? h->covered.p : nullptr;
-  // ---- grouped Schur lists (CCM_SCHUR=16 / 17): groups of QG consecutive off-diagonal upper blocks per row, entries built from the
-  // local observations; the pair lists below then hold the diagonal blocks only (every off-diagonal block marked as covered)
-  h->quad_built = (schur_mode() == 16 || schur_mode() == 17);
-  h->ng = 0;
-  if (h->quad_built) {
-    CCM_REQUIRE(!h->panel_on, "CCM_SCHUR=16/17 and CCM_SCHUR_PANEL are alternatives");
-    std::vector<int> grow((size_t)Kf + 1, 0), first, count;
-    for (int a2 = 0; a2 < Kf; a2++) {
-      const int u0 = h_udiag[a2] + 1, u1 = a2 + 1 < Kf ? h_udiag[a2 + 1] : nub;
-      for (int q = u0; q < u1; q += QG) { first.push_back(q); count.push_back(std::min(QG, u1 - q)); }
-      grow[a2 + 1] = (int)first.size();
-    }
-    h->ng = (int)first.size();
-    h->covered.alloc(std::max(nub, 1));
-    CCM_CUDA(cudaMemsetAsync(h->covered.p, 1, std::max(nub, 1), s));   // only read for off-diagonal blocks
-    cov = h->covered.p;
-    std::vector<unsigned> h_gp((size_t)h->ng + 1, 0);
-    if (h->ng > 0) { upload_vec(h->g_first, first, s); upload_vec(h->g_count, count, s); }
-    else { h->g_first.alloc(1); h->g_count.alloc(1); }
-    unsigned long long run = 0;
-    if (h->ng > 0 && El > 0) {
-      DevBuf<int> g_rowstart;
-      upload_vec(g_rowstart, grow, s);
-      DevBuf<unsigned> gcnt; gcnt.alloc_zero(h->ng, s);
-      k_quad_entries<<<div_up(El, TPB), TPB, 0, s>>>(h->o_kf.p, h->o_lm.p, h->lm_ptr.p, h->pose_slot.p, h->bitmap.p, h->word_prefix.p,
-                                                     h->s_rowptr.p, h->csr_u.p, words, El, 0, h->u_diag.p, g_rowstart.p, gcnt.p, nullptr, nullptr);
-      CCM_LAUNCHED();
-      std::vector<unsigned> c(h->ng);
-      gcnt.download(c.data(), h->ng, s);
-      CCM_CUDA(cudaStreamSynchronize(s));
-      for (int g = 0; g < h->ng; g++) { h_gp[g] = (unsigned)run; run += c[g]; }
-      CCM_REQUIRE(run < (1ull << 32) / (QG + 1), "too many grouped Schur entries for 32-bit offsets");
-      h_gp[h->ng] = (unsigned)run;
-      upload_vec(h->g_ptr, h_gp, s);
-      h->g_ent.alloc(std::max<size_t>((size_t)run * (QG + 1), 1));
-      if (run) {
-        CCM_CUDA(cudaMemsetAsync(gcnt.p, 0, sizeof(unsigned) * h->ng, s));
-        k_quad_entries<<<div_up(El, TPB), TPB, 0, s>>>(h->o_kf.p, h->o_lm.p, h->lm_ptr.p, h->pose_slot.p, h->bitmap.p, h->word_prefix.p,
-                                                       h->s_rowptr.p, h->csr_u.p, words, El, 1, h->u_diag.p, g_rowstart.p, gcnt.p, h->g_ptr.p, h->g_ent.p);
-        CCM_LAUNCHED();
-      }
-      CCM_CUDA(cudaStreamSynchronize(s));   // g_rowstart, gcnt and the host vectors die here
-    } else {
-      upload_vec(h->g_ptr, h_gp, s);
-      h->g_ent.alloc(1);
-      CCM_CUDA(cudaStreamSynchronize(s));
-    }
-    h->nquad = (long long)run;
-    if (sprof) fprintf(stderr, "[ccm_ba_create r%d] grouped Schur lists: %d groups, %lld entries\n", h->rank, h->ng, h->nquad);
-    lap("grouped product lists");
-  }
   // ---- Schur product lists (local shard)
   DevBuf<unsigned> counters; counters.alloc_zero(std::max(nub, 1), s);
   std::vector<unsigned> h_pp((size_t)nub + 1, 0);
   if (El && nub) {
     k_products<<<div_up(El, TPB), TPB, 0, s>>>(h->o_kf.p, h->o_lm.p, h->lm_ptr.p, h->pose_slot.p, h->bitmap.p,
                                                h->word_prefix.p, h->s_rowptr.p, h->csr_u.p, words, El, 0, counters.p,
-                                               nullptr, nullptr, cov);
+                                               nullptr, nullptr);
     CCM_LAUNCHED();
     std::vector<unsigned> c(nub);
     counters.download(c.data(), nub, s);
@@ -960,53 +755,8 @@ void build(ccm_ba_handle* h, const ccm_ba_problem* p) {
     CCM_CUDA(cudaMemsetAsync(counters.p, 0, sizeof(unsigned) * nub, s));
     k_products<<<div_up(El, TPB), TPB, 0, s>>>(h->o_kf.p, h->o_lm.p, h->lm_ptr.p, h->pose_slot.p, h->bitmap.p,
                                                h->word_prefix.p, h->s_rowptr.p, h->csr_u.p, words, El, 1, counters.p,
-                                               h->u_prod_ptr.p, h->prod.p, cov);
+                                               h->u_prod_ptr.p, h->prod.p);
     CCM_LAUNCHED();
-  }
-
-  // Sorted lists and T x T tiles did not beat the plain list kernel on cfg5 (large tiles lose: the long diagonal lists keep a
-  // 16-warp CTA alive while most warps idle) -- the gather is not L1-reuse bound.  Both stay available for experiments (CCM_SCHUR_SORT=1, CCM_SCHUR=9 + CCM_SCHUR_TILE) but cost set-up time, so they are off by default.
-  const bool want_tiles = schur_mode() == 9, want_rowsync = schur_mode() == 10;
-  if (h->nprod && env_int("CCM_SCHUR_SORT", (want_tiles || want_rowsync) ? 1 : 0)) {   // landmark order inside every list: deterministic sums
-    k_sort_products<<<nub, 256, 0, s>>>(h->u_prod_ptr.p, nub, h->prod.p);
-    CCM_LAUNCHED();
-  }
-  h->tile_T = env_int("CCM_SCHUR_TILE", 2);
-  h->ntiles = 0;
-  if (want_tiles && nub > 0 && h->nprod && (h->tile_T == 2 || h->tile_T == 3 || h->tile_T == 4)) {
-    // tile schedule: sort the upper blocks by (row group, column group), cut where the tile changes
-    DevBuf<unsigned long long> k_in, k_out;
-    DevBuf<int> v_in, v_out, head, rank;
-    k_in.alloc(nub); k_out.alloc(nub); v_in.alloc(nub); v_out.alloc(nub); head.alloc(nub); rank.alloc(nub);
-    const unsigned long long ngroups = (unsigned long long)(Kf / h->tile_T + 1);
-    k_tile_keys<<<div_up(nub, TPB), TPB, 0, s>>>(h->u_row.p, h->u_col.p, nub, h->tile_T, ngroups, k_in.p, v_in.p);
-    CCM_LAUNCHED();
-    size_t tb1 = 0, tb2 = 0;
-    CCM_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb1, k_in.p, k_out.p, v_in.p, v_out.p, nub, 0, 64, s));
-    CCM_CUDA(cub::DeviceScan::InclusiveSum(nullptr, tb2, head.p, rank.p, nub, s));
-    DevBuf<unsigned char> tmp; tmp.alloc(std::max(tb1, tb2) + 16);
-    CCM_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tb1, k_in.p, k_out.p, v_in.p, v_out.p, nub, 0, 64, s));
-    k_tile_heads<<<div_up(nub, TPB), TPB, 0, s>>>(k_out.p, nub, head.p);
-    CCM_LAUNCHED();
-    CCM_CUDA(cub::DeviceScan::InclusiveSum(tmp.p, tb2, head.p, rank.p, nub, s));
-    h->tile_ptr.alloc((size_t)nub + 1);
-    k_tile_ptr<<<div_up(nub, TPB), TPB, 0, s>>>(head.p, rank.p, nub, h->tile_ptr.p);
-    CCM_LAUNCHED();
-    h->tile_u.alloc(nub);
-    CCM_CUDA(cudaMemcpyAsync(h->tile_u.p, v_out.p, sizeof(int) * (size_t)nub, cudaMemcpyDeviceToDevice, s));
-    CCM_CUDA(cudaMemcpyAsync(&h->ntiles, rank.p + (nub - 1), sizeof(int), cudaMemcpyDeviceToHost, s));
-    CCM_CUDA(cudaStreamSynchronize(s));  // ntiles is the grid size; the temporaries die here
-  }
-  h->rs_ctas = 0;
-  if (want_rowsync && nub > 0 && h->nprod) {   // CTAs of <= RS_W consecutive off-diagonal blocks, cut at row boundaries (host: Kf rows)
-    std::vector<int> first, count;
-    for (int a2 = 0; a2 < Kf; a2++) {
-      const int u0 = h_udiag[a2] + 1, u1 = a2 + 1 < Kf ? h_udiag[a2 + 1] : nub;   // the diagonal block is the first upper block of its row
-      for (int q = u0; q < u1; q += RS_W) { first.push_back(q); count.push_back(std::min(RS_W, u1 - q)); }
-    }
-    h->rs_ctas = (int)first.size();
-    upload_vec(h->rs_first, first, s); upload_vec(h->rs_count, count, s);
-    CCM_CUDA(cudaStreamSynchronize(s));
   }
   lap("product lists");
   // ---- measurements: wait for their copy (one-rank path), validate the weights there, apply the edge flags
@@ -1048,7 +798,7 @@ void build(ccm_ba_handle* h, const ccm_ba_problem* p) {
     DevBuf<unsigned char> tmp; tmp.alloc(tb + 16);
     CCM_CUDA(cub::DeviceScan::InclusiveSum(tmp.p, tb, head.p, rank.p, Pl, s));
     h->units.alloc((size_t)Pl + 1);
-    k_tile_ptr<<<div_up(Pl, TPB), TPB, 0, s>>>(head.p, rank.p, Pl, h->units.p);   // units[rank - 1] = head, units[nunits] = Pl
+    k_unit_ptr<<<div_up(Pl, TPB), TPB, 0, s>>>(head.p, rank.p, Pl, h->units.p);   // units[rank - 1] = head, units[nunits] = Pl
     CCM_LAUNCHED();
     CCM_CUDA(cudaMemcpyAsync(&h->nunits, rank.p + (Pl - 1), sizeof(int), cudaMemcpyDeviceToHost, s));
     CCM_CUDA(cudaStreamSynchronize(s));   // nunits sizes the grids; the temporaries die here
@@ -1111,7 +861,7 @@ void build(ccm_ba_handle* h, const ccm_ba_problem* p) {
   if (Pl) CCM_CUDA(cudaMemcpyAsync(h->pt_trial, h->pt0.p, sizeof(double) * 3 * Pl, cudaMemcpyDeviceToDevice, s));
   h->pose_eval = h->pose_cur; h->pt_eval = h->pt_cur;
   CCM_CUDA(cudaStreamSynchronize(s));
-  h->device_bytes = (int64_t)(h->Z.bytes() +h->prod.bytes() + h->g_ent.bytes() + h->s_val.bytes() + h->Ubuf.bytes() +
+  h->device_bytes = (int64_t)(h->Z.bytes() + h->prod.bytes() + h->s_val.bytes() + h->Ubuf.bytes() +
                               h->bitmap.bytes() + h->word_prefix.bytes() + h->HllBl.bytes() + h->o_kf.bytes() * 2 +
                               h->o_uv.bytes() + h->o_w.bytes() * 2 + h->ptA.bytes() * 3);
   lap("storage + initial state");
@@ -1536,31 +1286,10 @@ extern "C" int ccm_ba_debug_schur_blocks(ccm_ba_handle* h, int32_t* rowptr, int3
 extern "C" int ccm_ba_debug_paths(ccm_ba_handle* h, int32_t* out) {
   return guarded([&] {
     CCM_REQUIRE(h && out, "null argument");
-    CCM_CUDA(cudaSetDevice(h->device));
-    int pan = 0, cov = 0;
-    if (h->panel_on) {
-      std::vector<unsigned char> po(h->npan), cv(h->nub);
-      h->pan_on.download(po.data(), po.size(), h->stream);
-      h->covered.download(cv.data(), cv.size(), h->stream);
-      CCM_CUDA(cudaStreamSynchronize(h->stream));
-      for (unsigned char c : po) pan += c;
-      for (unsigned char c : cv) cov += c;
-    }
-    out[0] = schur_path(h);
-    out[1] = pan;
-    out[2] = h->panel_on ? h->npan : 0;
-    out[3] = cov;
-    out[4] = h->p2.on ? 2 : 1;
-    out[5] = h->pcg_block;
-    out[6] = h->pcg_agg;
-    out[7] = h->pcg_nc;
-  });
-}
-
-extern "C" int ccm_ba_debug_set_schur_mode(int mode) {
-  return guarded([&] {
-    CCM_REQUIRE(mode >= -1 && mode <= 17, "ccm_ba_debug_set_schur_mode: -1 (CCM_SCHUR / default), 0 gather, 1 mma, 2..8 mma variants, 9 tiled, 10 row-synchronous, 11..15 vectorised entry loads, 16 / 17 grouped lists");
-    g_schur_override.store(mode);
+    out[0] = h->p2.on ? 2 : 1;
+    out[1] = h->pcg_block;
+    out[2] = h->pcg_agg;
+    out[3] = h->pcg_nc;
   });
 }
 

@@ -207,17 +207,17 @@ def make_local_ba(n_local=15, n_fixed=10, P=2000, obs_per_point=6, seed=1, name=
 
 
 def make_awkward_ba(seed=21) -> BAProblem:
-    """A global-BA problem built to sit on the edges of the Schur kernels' schedules (tests/test_gpu_schur.py asserts each feature):
-    199 free keyframes (not a multiple of the 8-row panel or of a 3 / 4 tile edge), fixed keyframes inside panels, co-observations
-    at free-pose offsets 43, 44 (the panel band edge) and beyond, landmarks with more than 160 observations (a panel stage cannot
-    hold them), runs of two-observation landmarks (stages capped at 32 landmarks), one keyframe pair sharing more than 4096
-    landmarks, a landmark only fixed keyframes see, one seen once, edges with flag bits 0 and 1, and observations in shuffled order.
+    """A global-BA problem built to sit on the edges of the Schur path's schedules (tests/test_gpu_schur.py checks it):
+    199 free keyframes, fixed keyframes among the free ones, co-observations at free-pose offsets 43, 44 and beyond, landmarks with
+    more than 160 observations (more than one 128-observation chunk of the landmark schedule), runs of two-observation landmarks,
+    one keyframe pair sharing more than 4096 landmarks, a landmark only fixed keyframes see, one seen once, edges with flag bits
+    0 and 1, and observations in shuffled order.
     The added landmarks are not geometrically consistent (only the linear system at the initial state is of interest)."""
     rng = np.random.default_rng(seed)
     p = make_global_ba(203, 3000, 6, window=50, n_agents=1, seed=seed)
     K = p.K
     fixed = np.zeros(K, np.uint8)
-    fixed[[0, 13, 50, 101]] = 1                       # 199 free; 13, 50 and 101 sit inside panels of the free poses
+    fixed[[0, 13, 50, 101]] = 1                       # 199 free; 13, 50 and 101 sit among the free poses
     free_idx = np.flatnonzero(fixed == 0)
     obs = [(p.obs_kf, p.obs_mp, p.obs_uv, p.obs_w)]
     pts = [p.points]
@@ -236,9 +236,9 @@ def make_awkward_ba(seed=21) -> BAProblem:
         nxt += 1
 
     a = free_idx[30]
-    for d in (43, 44, 47, 60):                        # free-pose offsets at and beyond the band edge
+    for d in (43, 44, 47, 60):                        # co-observations at growing free-pose offsets
         add([a, free_idx[30 + d]])
-    for _ in range(2):                                # more observations than a panel stage holds
+    for _ in range(2):                                # more observations than a chunk of the landmark schedule
         add(np.sort(rng.choice(np.arange(20, 200), 170, replace=False)))
     for _ in range(4200):                             # one pair of keyframes sharing > 4096 landmarks, as two-observation landmarks
         add([free_idx[70], free_idx[71]])

@@ -150,7 +150,7 @@ int ccm_ba_get_info(const ccm_ba_handle* h, ccm_ba_info* info);
                                   launches in the first iteration and after a rejected trial) */
 #define CCM_BA_K_POSE_PASS 1   /* k_pose_pass: Hpp/bp                                            (per LM iteration) */
 #define CCM_BA_K_SCALE 2       /* no kernel: Z is formed by k_linearize (slot kept, records no launches) */
-#define CCM_BA_K_SCHUR 3       /* k_schur: Schur products                                        (per LM trial) */
+#define CCM_BA_K_SCHUR 3       /* k_schur_mma: Schur products                                    (per LM trial) */
 #define CCM_BA_K_ALLREDUCE 4   /* NCCL all-reduce of [S upper | bschur part]                     (per LM trial, N>1) */
 #define CCM_BA_K_FINALIZE 5    /* k_finalize_S + k_block_jacobi                                  (per LM trial) */
 #define CCM_BA_K_PCG 6         /* k_pcg (persistent)                                             (per LM trial) */
@@ -173,14 +173,9 @@ int ccm_ba_debug_schur(ccm_ba_handle* h, int robust, double huber_delta, double 
  * nnzb = ccm_ba_info.s_blocks_full.  Any output may be NULL. */
 int ccm_ba_debug_schur_blocks(ccm_ba_handle* h, int32_t* rowptr /*K+1*/, int32_t* col /*nnzb*/, double* val /*nnzb*36*/,
                               double* bschur /*6K*/);
-/* the paths the handle runs: out[0] Schur mode in effect (CCM_SCHUR numbering; 9 / 10 without their schedule run as 8),
- * out[1] panels enabled, out[2] panels in total (0 without CCM_SCHUR_PANEL), out[3] upper blocks the panels own,
- * out[4] PCG implementation (1 k_pcg, 2 k_pcg2), out[5] k_pcg CTA size, out[6] coarse aggregate size, out[7] coarse nodes (0: no coarse space) */
-int ccm_ba_debug_paths(ccm_ba_handle* h, int32_t* out /*8*/);
-/* developer hook: pick the Schur-product kernel for every handle of this process: 0 = gather form (k_schur), 1 = tensor-core
- * form (k_schur_mma, one f64 mma.sync per product; the default), 2..8 = variants of it (unroll 16 / 4, CTA 64 / 256 / 512, entry prefetch; the default is unroll 8, CTA 128),
- * -1 = back to the CCM_SCHUR environment variable / built-in default */
-int ccm_ba_debug_set_schur_mode(int mode);
+/* the PCG path the handle runs: out[0] implementation (1 k_pcg, 2 k_pcg2), out[1] k_pcg CTA size, out[2] coarse aggregate size,
+ * out[3] coarse nodes (0: no coarse space) */
+int ccm_ba_debug_paths(ccm_ba_handle* h, int32_t* out /*4*/);
 /* time `reps` launches of one kernel with CUDA events on the handle's stream; returns mean ms per launch.
  * which: 0 linearize (landmark pass, Hll/bl and Z), 1 pose pass, 2 residual/chi2, 3 Z-only linearize (g and Z at lambda),
  * 4 schur products, 5 back-substitution */

@@ -1,8 +1,7 @@
-"""The reduced camera system on the GPU, block by block: every Schur kernel variant (CCM_SCHUR 0-17, sorted lists, tile edges, the
-landmark-synchronous panels) against the f64 restatement of tests/schur_ref.py, fed with the device's own linear system
-(ccm_ba_debug_build) so that only k_scale, the Schur kernels, k_finalize_S, k_block_jacobi, the solve and k_backsub_points are
-under test.  Every entry of S and b_schur, and every landmark step, is held to its own bound (TAU = 1e-12 times the absolute
-sum of its terms); a failure names the configuration and the worst block."""
+"""The reduced camera system on the GPU, block by block: the Schur product kernel (k_schur_mma) against the f64 restatement of
+tests/schur_ref.py, fed with the device's own linear system (ccm_ba_debug_build) so that only the Z pass, the Schur kernel,
+k_finalize_S, k_block_jacobi, the solve and k_backsub_points are under test.  Every entry of S and b_schur, and every landmark
+step, is held to its own bound (TAU = 1e-12 times the absolute sum of its terms); a failure names the case and the worst block."""
 import numpy as np
 import pytest
 
@@ -19,20 +18,6 @@ SHAPES = {
     "cfg5_tenth": lambda: synth.make_config("cfg5", K=1000, P=100000),
     "awkward": synth.make_awkward_ba,
 }
-LIST_MODES = [m for m in range(18) if m not in (9, 10, 16, 17)]   # share one handle: the mode is read at launch
-BIG = "1000000"
-
-
-def _configs():
-    """(label, mode, env, fresh handle)"""
-    c = [(f"mode{m}", m, {}, False) for m in LIST_MODES]
-    c += [(f"mode{m}", m, {}, True) for m in (9, 10, 16, 17)]
-    c += [(f"mode{m}+sort", m, {"CCM_SCHUR_SORT": "1"}, True) for m in list(range(1, 9)) + list(range(11, 16))]
-    c += [(f"mode9+tile{t}", 9, {"CCM_SCHUR_TILE": str(t)}, True) for t in (3, 4)]
-    for fac in ("default", "all"):
-        env = {"CCM_SCHUR_PANEL": "1"} if fac == "default" else {"CCM_SCHUR_PANEL": "1", "CCM_SCHUR_PANEL_FACTOR": BIG}
-        c += [(f"panel-{fac}+mode{m}", m, env, True) for m in range(16)]
-    return c
 
 
 @pytest.fixture(scope="module", autouse=True)
@@ -64,74 +49,31 @@ def _run(h, lam, robust):
     return got, blk
 
 
-def _check(ref, got, blk, label, table):
+def _check(ref, got, blk, label):
     r = R.compare_blocks(ref, blk)
     d, dt = ref.dx_point(got["dx_pose"])
     r["dx_point"] = R.ratio(got["dx_point"] - d, dt)
-    table.append((label, r))
     worst = R.worst_block(ref, blk)
     return r, f"{label}: err/tol {r}, worst block (row {worst[0]}, col {worst[1]}) at {worst[2]:.3g}"
-
-
-def _expect_path(label, mode, env, paths):
-    assert paths["schur_mode"] == mode, (label, paths)
-    if env.get("CCM_SCHUR_PANEL"):
-        assert paths["panels"] > 0, (label, paths)
-        if env.get("CCM_SCHUR_PANEL_FACTOR") == BIG:   # every panel on, and they own blocks
-            assert paths["panels_on"] == paths["panels"] and paths["covered"] > 0, (label, paths)
-    else:
-        assert paths["panels"] == 0 and paths["covered"] == 0, (label, paths)
 
 
 @pytest.mark.parametrize("robust", [True, False], ids=["robust", "plain"])
 @pytest.mark.parametrize("lam_kind", ["lm_start", "heavy"])
 @pytest.mark.parametrize("name", list(SHAPES))
-def test_every_schur_variant_matches_the_restatement(name, lam_kind, robust, monkeypatch, capsys):
+def test_schur_kernel_matches_the_restatement(name, lam_kind, robust, capsys):
     p, b, md = _case(name, robust)
     lam = (1e-5 if lam_kind == "lm_start" else 1e-1) * md
     ref = R.schur_reference(p, b, lam)
-    table, fails = [], []
-    shared = None
-    with api.schur_mode(11):
-        shared = api.BAHandle(p)
+    label = f"{name} {lam_kind} {'robust' if robust else 'plain'}"
+    h = api.BAHandle(p)
     try:
-        for label, mode, env, fresh in _configs():
-            with monkeypatch.context() as mp:
-                for k, v in env.items():
-                    mp.setenv(k, v)
-                with api.schur_mode(mode):
-                    if mode in (16, 17) and env.get("CCM_SCHUR_PANEL"):
-                        continue
-                    if env.get("CCM_SCHUR_PANEL") and p.K - int(p.fixed.sum()) < 1:
-                        continue
-                    h = api.BAHandle(p) if fresh else shared
-                    try:
-                        paths = h.debug_paths()
-                        if not (name == "tiny" and mode in (9, 10)):   # tiny: the row / tile schedule may be empty
-                            _expect_path(label, mode, env, paths)
-                        got, blk = _run(h, lam, robust)
-                    finally:
-                        if fresh:
-                            h.close()
-                r, msg = _check(ref, got, blk, label, table)
-                if max(r.values()) > 1.0:
-                    fails.append(msg)
+        got, blk = _run(h, lam, robust)
     finally:
-        shared.close()
+        h.close()
+    r, msg = _check(ref, got, blk, label)
     with capsys.disabled():
-        worst = max(table, key=lambda t: max(t[1].values()))
-        print(f"\n[schur {name} {lam_kind} {'robust' if robust else 'plain'}] {len(table)} variants, "
-              f"max err/tol S {max(t[1]['S'] for t in table):.3g} b {max(t[1]['bschur'] for t in table):.3g} "
-              f"dx {max(t[1]['dx_point'] for t in table):.3g} (worst: {worst[0]})")
-    assert not fails, "\n".join(fails)
-
-
-@pytest.mark.parametrize("mode", [16, 17])
-def test_grouped_lists_with_panels_are_refused(mode, monkeypatch):
-    monkeypatch.setenv("CCM_SCHUR_PANEL", "1")
-    with api.schur_mode(mode):
-        with pytest.raises(api.CCMError, match="alternatives"):
-            api.BAHandle(synth.make_config("small"))
+        print(f"\n[schur {label}] err/tol S {r['S']:.3g} b {r['bschur']:.3g} dx {r['dx_point']:.3g}")
+    assert max(r.values()) <= 1.0, msg
 
 
 @pytest.mark.parametrize("name", ["tiny", "small"])
