@@ -390,9 +390,11 @@ __global__ void __launch_bounds__(1024) k_sum_partials(const double* __restrict_
 // i.e. 18 lanes x 8 B per operand (2 cache lines), no cross-lane reduction.  Diagonal blocks put g_l into B's column 6, so
 // C[r][6] = sum_o Z_o[r][:] . g_l(o) = bneg comes out of the same instruction.  Two accumulator sets (products alternate) keep
 // two MMA chains in flight; they are added in a fixed order: deterministic per list order.
-// The kernel is bound by the L1 data pipe's wavefront rate, so the UNROLL list entries of a batch come in with ONE coalesced load
-// (lane j takes entry j) and reach the other lanes by shuffle, instead of UNROLL broadcast loads.  Off-diagonal blocks request the
-// entries of batch k+1 before the rows of batch k, so the entry -> row dependence costs one memory latency per batch instead of two.
+// The UNROLL list entries of a batch come in with ONE coalesced load (lane j takes entry j) and reach the other lanes by shuffle,
+// instead of UNROLL broadcast loads.  Off-diagonal blocks request the entries of batch k+1 before the rows of batch k, so the
+// entry -> row dependence costs one memory latency per batch instead of two.  On H100 the kernel is bound by the rows it keeps in
+// flight: the 2 * UNROLL rows of a batch are requested together, and UNROLL 16 at 66 registers runs a cfg5 launch in 9.6 ms against
+// 11.3 at UNROLL 8 (48 registers), 10.0 at 32 and 12.7 at 4 (H100 80GB HBM3, 700 W).
 __device__ __forceinline__ void dmma_884(double& c0, double& c1, double a, double b) {
   asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};"
                : "+d"(c0), "+d"(c1)
@@ -405,7 +407,7 @@ __global__ void __launch_bounds__(SCHUR_CTA) k_schur_mma(const uint2* __restrict
                                                          const double* __restrict__ Z, const int* __restrict__ o_lm,
                                                          const double* __restrict__ gvec, double* __restrict__ U_val,
                                                          double* __restrict__ bneg) {
-  constexpr int UNROLL = 8;   // products per batch; even: they alternate between the two accumulator sets
+  constexpr int UNROLL = 16;  // products per batch; even: they alternate between the two accumulator sets; <= 32 (one entry per lane)
   const int warp = (int)(((long long)blockIdx.x * SCHUR_CTA + threadIdx.x) >> 5);
   if (warp >= nub) return;  // warp-uniform
   const int lane = threadIdx.x & 31;
