@@ -278,6 +278,14 @@ class BAHandle:
         _chk(lib().ccm_ba_debug_paths(self._h, _p(out)))
         return {k: int(v) for k, v in zip(self.PATH_KEYS, out)}
 
+    def debug_coarse(self):
+        """the coarse level of the PCG preconditioner on the S the last debug_schur left: the assembled Galerkin matrix P^T S P
+        and its inverse from the PCG set-up, both (6 nc, 6 nc)"""
+        nC = 6 * self.debug_paths()["pcg_nc"]
+        Ac = np.empty((nC, nC)); Ainv = np.empty((nC, nC))
+        _chk(lib().ccm_ba_debug_coarse(self._h, _p(Ac), _p(Ainv)))
+        return dict(Ac=Ac, Ainv=Ainv)
+
     def set_estimate(self, poses=None, points=None):
         """replace the estimate, keep structure and observations on the device (ccm_ba_set_estimate)"""
         ps = None if poses is None else np.ascontiguousarray(poses, np.float64)

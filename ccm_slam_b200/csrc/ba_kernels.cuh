@@ -394,12 +394,7 @@ __global__ void __launch_bounds__(1024) k_sum_partials(const double* __restrict_
 // instead of UNROLL broadcast loads.  Off-diagonal blocks request the entries of batch k+1 before the rows of batch k, so the
 // entry -> row dependence costs one memory latency per batch instead of two.  On H100 the kernel is bound by the rows it keeps in
 // flight: the 2 * UNROLL rows of a batch are requested together, and UNROLL 16 at 66 registers runs a cfg5 launch in 9.6 ms against
-// 11.3 at UNROLL 8 (48 registers), 10.0 at 32 and 12.7 at 4 (H100 80GB HBM3, 700 W).
-__device__ __forceinline__ void dmma_884(double& c0, double& c1, double a, double b) {
-  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};"
-               : "+d"(c0), "+d"(c1)
-               : "d"(a), "d"(b));
-}
+// 11.3 at UNROLL 8 (48 registers), 10.0 at 32 and 12.7 at 4 (H100 80GB HBM3, 700 W).  (dmma_884: pcg.cuh)
 
 constexpr int SCHUR_CTA = 128;   // threads per CTA of k_schur_mma: 4 upper blocks
 __global__ void __launch_bounds__(SCHUR_CTA) k_schur_mma(const uint2* __restrict__ prod, const unsigned* __restrict__ u_prod_ptr,

@@ -270,10 +270,7 @@ void step_finalize(ccm_ba_handle* h, double lambda) {
   CCM_LAUNCHED();
 }
 
-void step_pcg(ccm_ba_handle* h, double tol, int max_iter) {
-  cudaStream_t s = h->stream;
-  KernelSpan sp(h, CCM_BA_K_PCG);
-  CCM_CUDA(cudaMemsetAsync(h->pcg_bar.p, 0, 2 * sizeof(unsigned), s));
+PcgArgs pcg_args(ccm_ba_handle* h, double tol, int max_iter) {
   PcgArgs a;
   a.n = h->Kf; a.rowptr = h->s_rowptr.p; a.col = h->s_col.p; a.val = h->s_val.p; a.Minv = h->Minv.p; a.b = h->bschur.p;
   a.x = h->x.p; a.r = h->pr.p; a.z = h->pz.p; a.p = h->pp.p; a.q = h->pq.p;
@@ -281,6 +278,14 @@ void step_pcg(ccm_ba_handle* h, double tol, int max_iter) {
   a.agg = h->pcg_agg; a.nc = h->pcg_nc; a.Ac = h->pcg_Ac.p; a.rc = h->pcg_rc.p; a.yc = h->pcg_yc.p;
   a.prof = h->pcg_prof.p;
   a.prolong = h->pcg_prolong;
+  return a;
+}
+
+void step_pcg(ccm_ba_handle* h, double tol, int max_iter) {
+  cudaStream_t s = h->stream;
+  KernelSpan sp(h, CCM_BA_K_PCG);
+  CCM_CUDA(cudaMemsetAsync(h->pcg_bar.p, 0, 2 * sizeof(unsigned), s));
+  PcgArgs a = pcg_args(h, tol, max_iter);
   a.coarse_mode = (h->pcg_coarse_valid && h->pcg_age < h->pcg_refresh) ? 2 : 1;
   h->pcg_last_mode = a.coarse_mode;
   if (h->p2.on) {
@@ -298,7 +303,7 @@ void step_pcg(ccm_ba_handle* h, double tol, int max_iter) {
     b.Minv = h->Minv.p; b.b = h->bschur.p; b.x = h->x.p; b.r = h->pr.p; b.q = h->pq.p; b.p = h->pp.p;
     b.partials = h->pcg_partials.p; b.bar = h->pcg_bar.p; b.tol = tol; b.max_iter = max_iter; b.status = h->pcg_status.p;
     b.agg = a.agg; b.nc = a.nc; b.prolong = a.prolong;
-    b.Ainv = nC > 0 ? ((((nC + GJB - 1) / GJB) & 1) ? h->pcg_Ac.p + (size_t)nC * nC : h->pcg_Ac.p) : nullptr;
+    b.Ainv = nC > 0 ? coarse_inverse(h->pcg_Ac.p, nC) : nullptr;
     b.yc = d.yc.p; b.tpart = d.tpart.p;
     b.rank = h->rank; b.nranks = h->nranks; b.r0 = d.r0; b.r1 = d.r1; b.win = d.d_win.p;
     b.off_z = d.lay.off_z; b.off_x = d.lay.off_x;
@@ -836,15 +841,16 @@ void build(ccm_ba_handle* h, const ccm_ba_problem* p) {
   h->pcg_partials.alloc((size_t)3 * h->pcg_grid);
   if (env_int("CCM_PCG_PROF", 0)) h->pcg_prof.alloc_zero(8, s);
   // coarse space: <= 128 aggregates for small systems, <= 384 for long trajectories where the smooth modes dominate the
-  // iteration count; the inverse is refreshed every 2nd / 4th solve (measured sweeps: tools/ba_probe.py with CCM_PCG_NC/REFRESH)
+  // iteration count; the inverse is refreshed every 2nd solve (measured sweeps: tools/ba_probe.py with CCM_PCG_NC/REFRESH)
   // CCM_PCG_PROLONG=1: piecewise-linear prolongation (pcg.cuh); half the coarse nodes then already beat the constant P
   h->pcg_prolong = env_int("CCM_PCG_PROLONG", 1) ? 1 : 0;  // cfg5: 1538 -> 617 PCG iterations per Global BA at 192 coarse nodes
   // PCG iterations per Global BA on cfg5: NC 192 refresh 4: 617, NC 192 refresh 2: 545, NC 256 refresh 2: 400, NC 256 refresh 1: 384,
   // NC 384 refresh 4: 357 (its 2304^2 inverse is the most expensive), NC 128 refresh 1: 1014; refresh 8 (one inverse per BA): 1950
   pcg_coarse_shape(Kf, env_int("CCM_PCG_NC", Kf >= 4096 ? (h->pcg_prolong ? 256 : 384) : 128), &h->pcg_agg, &h->pcg_nc);
-  // refresh 2 / 3 / 4 with NC 256: 400 / 427 / 496 iterations, but fewer inversions; the solve time is flat over them, so the
-  // large systems take the fewest inversions (the inverse is replicated work on several ranks); small systems keep 2
-  h->pcg_refresh = std::max(1, env_int("CCM_PCG_REFRESH", Kf >= 4096 ? 4 : 2));
+  // refresh 1 / 2 / 4 with NC 256: 384 / 400 / 496 iterations per cfg5 Global BA.  An iteration of k_pcg2 costs about 120 us and
+  // the set-up launch that rebuilds the 1536^2 inverse 2.0 ms, so one BA takes 173 / 167 / 174 ms; cfg4 (k_pcg, nC = 690) takes
+  // 27.3 / 24.5 ms at refresh 1 / 2 (H100 80GB HBM3, 700 W).  Every size rebuilds every 2nd solve.
+  h->pcg_refresh = std::max(1, env_int("CCM_PCG_REFRESH", 2));
   {
     const size_t nC = (size_t)6 * h->pcg_nc;
     h->pcg_Ac.alloc(std::max(2 * nC * nC, (size_t)1)); h->pcg_rc.alloc(std::max(2 * nC, (size_t)1)); h->pcg_yc.alloc(std::max(nC, (size_t)1));
@@ -1280,6 +1286,30 @@ extern "C" int ccm_ba_debug_schur_blocks(ccm_ba_handle* h, int32_t* rowptr, int3
       memset(bschur, 0, sizeof(double) * 6 * (size_t)K);
       for (int a = 0; a < Kf; a++) memcpy(bschur + 6 * (size_t)h->h_slot_pose[a], hb.data() + (size_t)a * 6, 6 * sizeof(double));
     }
+  });
+}
+
+extern "C" int ccm_ba_debug_coarse(ccm_ba_handle* h, double* Ac, double* Ainv) {
+  return guarded([&] {
+    CCM_REQUIRE(h && Ac && Ainv, "null argument");
+    CCM_REQUIRE(h->pcg_agg > 0 && h->pcg_nc > 0, "the handle has no coarse space");
+    cudaStream_t s = h->stream;
+    const int nC = 6 * h->pcg_nc;
+    const size_t bytes = (size_t)nC * nC * sizeof(double);
+    PcgArgs a = pcg_args(h, 0.0, 0);
+    for (int mode : {3, 1}) {  // the assembled matrix, then the set-up launch step_pcg makes before k_pcg2
+      a.coarse_mode = mode;
+      CCM_CUDA(cudaMemsetAsync(h->pcg_bar.p, 0, 2 * sizeof(unsigned), s));
+      void* args[] = {&a};
+      CCM_CUDA(cudaLaunchCooperativeKernel(h->pcg_fn, dim3(h->pcg_grid), dim3(h->pcg_block), args, 0, s));
+      CCM_LAUNCHED();
+      CCM_CUDA(cudaMemcpyAsync(mode == 3 ? Ac : Ainv, mode == 3 ? h->pcg_Ac.p : coarse_inverse(h->pcg_Ac.p, nC), bytes,
+                               cudaMemcpyDeviceToHost, s));
+    }
+    CCM_CUDA(cudaStreamSynchronize(s));
+    double st[4];
+    CCM_CUDA(cudaMemcpy(st, h->pcg_status.p, sizeof(st), cudaMemcpyDeviceToHost));
+    CCM_REQUIRE(st[3] > 0.0, "the coarse matrix has a non-positive pivot");
   });
 }
 

@@ -21,9 +21,27 @@
 namespace ccm {
 
 constexpr int TPB = 256;
-constexpr int GJB = 8;          // pivots eliminated per sweep of the coarse-matrix inversion (16 measured no faster: the per-row coefficient set-up grows with GJB^2)
-constexpr int GJ_CW = 256;       // column chunk a CTA stages per sweep
+// Coarse-matrix inversion: GJB pivots per Gauss-Jordan sweep, so one grid barrier and one pass over the matrix per GJB pivots.
+// Both products of a sweep run on the f64 tensor cores.  On cfg5 (nC = 1536: 48 sweeps) the set-up launch (assembly + inverse)
+// takes 2.0 ms; at 8 pivots per sweep on the CUDA cores it took 4.9 ms (H100 80GB HBM3, 700 W).
+constexpr int GJB = 32;
+constexpr int GJ_CW = 128;     // column chunk a CTA stages per sweep
+constexpr int GJ_LDP = GJB + 4;     // padded row strides of the shared pivot inverse / pivot rows: the B fragments of
+constexpr int GJ_LDR = GJ_CW + 4;   // mma.m8n8k4 read 4 rows x 8 columns, unpadded those 4 rows fall into the same banks
 constexpr int PCG_TPB = 1024;  // one fat CTA per SM keeps the grid barrier at one participant per SM (132 on an H100 SXM)
+
+// The ping-pong buffer of Ac (2 (BS nc)^2 doubles) that holds the coarse inverse after the set-up: the sweep count's parity.
+__host__ __device__ inline double* coarse_inverse(double* Ac, int nC) {
+  return (((nC + GJB - 1) / GJB) & 1) ? Ac + (size_t)nC * nC : Ac;
+}
+
+// D += A B on one 8x8x4 f64 tensor-core tile.  A (8x4 row-major): lane t holds A[t/4][t%4]; B (4x8 col-major): lane t holds
+// B[t%4][t/4]; C / D (8x8): lane t holds C[t/4][2 (t%4)] and C[t/4][2 (t%4) + 1].
+__device__ __forceinline__ void dmma_884(double& c0, double& c1, double a, double b) {
+  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0, %1}, {%2}, {%3}, {%0, %1};"
+               : "+d"(c0), "+d"(c1)
+               : "d"(a), "d"(b));
+}
 
 __device__ __forceinline__ double warp_sum(double v) {
 #pragma unroll
@@ -56,7 +74,8 @@ struct PcgArgs {
   double* status;    // [iters, relres, flag(0 converged, 1 max_iter, 2 breakdown: p'Sp <= 0), coarse_used]
   // coarse level (agg <= 0 disables it)
   int agg, nc;       // rows per aggregate, number of aggregates
-  int coarse_mode;   // 1: assemble + invert now, 2: reuse the inverse a previous launch left in Ac (still a valid SPD preconditioner)
+  int coarse_mode;   // 1: assemble + invert now, 2: reuse the inverse a previous launch left in Ac (still a valid SPD preconditioner),
+                     // 3: assemble into Ac and return (debug export)
   int prolong = 0;   // 0: piecewise-constant prolongation (one coarse node per aggregate), 1: piecewise linear between aggregate centres
   double* Ac;        // 2 * (BS*nc)^2 ping-pong buffers
   double* rc;        // 2 * BS*nc restricted residual (double buffered)
@@ -110,8 +129,9 @@ template <int BS, int MAXT = PCG_TPB, int MINB = 1>
 __global__ void __launch_bounds__(MAXT, MINB) k_pcg(PcgArgs A) {
   constexpr int BB = BS * BS;
   __shared__ double red[PCG_TPB / 32];
-  __shared__ double gj_rows[GJB * GJ_CW];
-  __shared__ double gj_pi[GJB * GJB];
+  __shared__ double gj_rows[GJB * GJ_LDR];
+  __shared__ double gj_pi[GJB * GJ_LDP];
+  __shared__ double gj_vr[2][GJB], gj_vc[2][GJB];
   __shared__ int gj_bad;
   const int bdim = blockDim.x;  // 256 (small systems: spread over more SMs) or PCG_TPB
   const int lane = threadIdx.x & 31;
@@ -129,7 +149,7 @@ __global__ void __launch_bounds__(MAXT, MINB) k_pcg(PcgArgs A) {
 
   // ---- coarse level set-up: Ac = P^T S P, then Ac^-1 by ping-pong Gauss-Jordan -------------------------------------
   if (coarse && A.coarse_mode == 2) {
-    Ainv = (((nC + GJB - 1) / GJB) & 1) ? A.Ac + (size_t)nC * nC : A.Ac;
+    Ainv = coarse_inverse(A.Ac, nC);
     for (long long i = gtid; i < 2ll * nC; i += gthreads) A.rc[i] = 0.0;
     grid_barrier(A.bar, target);
   } else if (coarse) {
@@ -204,106 +224,137 @@ __global__ void __launch_bounds__(MAXT, MINB) k_pcg(PcgArgs A) {
       }
     }
     grid_barrier(A.bar, target);
+    if (A.coarse_mode == 3) return;  // assembly only (ccm_ba_debug_coarse): A0 holds P^T S P
     // Block Gauss-Jordan without pivoting (the matrix is SPD, so every pivot block is too): sweep t eliminates GJB pivots at
-    // once (rank-GJB update), reads buffer t&1 and writes buffer (t+1)&1 -> one grid barrier and one pass over the matrix
-    // per GJB pivots instead of per pivot.  With A = [[P, R], [C, D]] the sweep writes [[P^-1, P^-1 R], [-C P^-1, D - C P^-1 R]].
-    // Work split of one sweep: the matrix is cut into column chunks of GJ_CW; a CTA stages the GJB pivot rows of its chunk
-    // in shared memory once and its warps stream rows i through it (read src[i][chunk], write dst[i][chunk]); the L2
-    // traffic per sweep is one read + one write of the matrix.
+    // once (rank-GJB update), reads buffer t&1 and writes buffer (t+1)&1.  With A = [[P, R], [C, D]] the sweep writes
+    // [[P^-1, P^-1 R], [-C P^-1, D - C P^-1 R]], one formula for every entry:
+    //   dst[i][j] = base[i][j] + H[i] . Rr[:, j],   H[i] = X[i] P^-1,
+    //   X[i] = -src[i][piv] (pivot rows: the unit vector e_{i-k0}),  Rr[l][j] = src[k0+l][j] (pivot columns: delta(l, j-k0)),
+    //   base = src off the pivot rows and columns, 0 on them.
+    // Both products run as mma.m8n8k4.f64 tiles, one warp per slab of 8 rows.  Work split of one sweep: the matrix is cut into
+    // column chunks of GJ_CW; a CTA stages Rr of its chunk in shared memory and its warps stream slabs through it (H is formed
+    // again per chunk: GJB / GJ_CW more flops, no extra barrier); the L2 traffic per sweep is about one read + one write of
+    // the matrix.
     bool bad = false;
     int sweep = 0;
     const int wid = threadIdx.x >> 5, wpc = bdim >> 5;
+    const int qr = lane >> 2, qc = lane & 3;  // mma fragment coordinates (see dmma_884)
     const int nch = (nC + GJ_CW - 1) / GJ_CW;
     const int rgs = G / nch > 0 ? G / nch : 1;  // CTAs sharing one column chunk
+    const int nslab = (nC + 7) >> 3;
+    constexpr int PE = (GJB * GJB + MAXT - 1) / MAXT;  // pivot-block entries per thread (every launch uses MAXT threads)
     for (int k0 = 0; k0 < nC; k0 += GJB, sweep++) {
       const int kb = nC - k0 < GJB ? nC - k0 : GJB;
       const double* src = (sweep & 1) ? A1 : A0;
       double* dst = (sweep & 1) ? A0 : A1;
-      if (wid == 0) {  // warp 0: inverse of the pivot block in shared memory (identical in every CTA); identity past kb
-        for (int t = lane; t < GJB * GJB; t += 32) {
-          const int a = t / GJB, b2 = t % GJB;
-          gj_pi[t] = (a < kb && b2 < kb) ? __ldcg(src + (size_t)(k0 + a) * nC + k0 + b2) : (a == b2 ? 1.0 : 0.0);
-        }
-        if (lane == 0) gj_bad = 0;
-        __syncwarp();
-        for (int q = 0; q < GJB; q++) {
-          const double piv = gj_pi[q * GJB + q];
-          const double ip = 1.0 / piv;
-          double nv[(GJB * GJB + 31) / 32];
+      // P^-1 (identity past kb) by Gauss-Jordan, identical in every CTA: each thread keeps its entries in registers, the
+      // pivot row and column of the next step go through the ping-pong vectors gj_vr / gj_vc -> one __syncthreads per pivot
+      double e[PE];
 #pragma unroll
-          for (int u = 0; u < (GJB * GJB + 31) / 32; u++) {
-            const int t = lane + 32 * u, r2 = t / GJB, c2 = t % GJB;
-            if (t < GJB * GJB) {
-              const double old = gj_pi[t], prq = gj_pi[r2 * GJB + q], pqc = gj_pi[q * GJB + c2];
-              nv[u] = r2 == q ? (c2 == q ? ip : pqc * ip) : (c2 == q ? -prq * ip : old - prq * (pqc * ip));
-            }
+      for (int u = 0; u < PE; u++) {
+        const int t = threadIdx.x + u * bdim, r2 = t / GJB, c2 = t % GJB;
+        e[u] = 0.0;
+        if (t < GJB * GJB) {
+          e[u] = (r2 < kb && c2 < kb) ? __ldcg(src + (size_t)(k0 + r2) * nC + k0 + c2) : (r2 == c2 ? 1.0 : 0.0);
+          if (r2 == 0) gj_vr[0][c2] = e[u];
+          if (c2 == 0) gj_vc[0][r2] = e[u];
+        }
+      }
+      if (threadIdx.x == 0) gj_bad = 0;
+      __syncthreads();
+      for (int q = 0; q < kb; q++) {  // the identity past kb has unit pivots and changes nothing
+        const double* vr = gj_vr[q & 1];
+        const double* vc = gj_vc[q & 1];
+        const double piv = vr[q];
+        const double ip = 1.0 / piv;
+#pragma unroll
+        for (int u = 0; u < PE; u++) {
+          const int t = threadIdx.x + u * bdim, r2 = t / GJB, c2 = t % GJB;
+          if (t < GJB * GJB) {
+            const double prq = vc[r2], pqc = vr[c2];
+            e[u] = r2 == q ? (c2 == q ? ip : pqc * ip) : (c2 == q ? -prq * ip : e[u] - prq * (pqc * ip));
+            if (r2 == q + 1) gj_vr[(q + 1) & 1][c2] = e[u];
+            if (c2 == q + 1) gj_vc[(q + 1) & 1][r2] = e[u];
           }
-          __syncwarp();
-#pragma unroll
-          for (int u = 0; u < (GJB * GJB + 31) / 32; u++)
-            if (lane + 32 * u < GJB * GJB) gj_pi[lane + 32 * u] = nv[u];
-          if (lane == 0 && (!(piv > 0.0) || !isfinite(piv))) gj_bad = 1;
-          __syncwarp();
         }
+        if (threadIdx.x == 0 && (!(piv > 0.0) || !isfinite(piv))) gj_bad = 1;
+        __syncthreads();
+      }
+      if (gj_bad) { bad = true; break; }  // uniform over the grid: every CTA inverted the same pivot block
+#pragma unroll
+      for (int u = 0; u < PE; u++) {
+        const int t = threadIdx.x + u * bdim;
+        if (t < GJB * GJB) gj_pi[(t / GJB) * GJ_LDP + t % GJB] = e[u];
       }
       for (int item = blockIdx.x; item < nch * rgs; item += G) {
         const int c0 = (item % nch) * GJ_CW, rg = item / nch;
         for (int t = threadIdx.x; t < GJB * GJ_CW; t += bdim) {
           const int l = t / GJ_CW, j = c0 + t % GJ_CW;
-          gj_rows[t] = (l < kb && j < nC) ? __ldcg(src + (size_t)(k0 + l) * nC + j) : 0.0;
+          gj_rows[l * GJ_LDR + t % GJ_CW] = (l >= kb || j >= nC) ? 0.0
+                                            : (j >= k0 && j < k0 + kb) ? (j - k0 == l ? 1.0 : 0.0)
+                                                                       : __ldcg(src + (size_t)(k0 + l) * nC + j);
         }
-        const int rstep = rgs * wpc;
-        int i = rg * wpc + wid;
-        double fn[GJB];  // pivot-column entries of the next row, fetched one row ahead
+        __syncthreads();  // gj_rows and gj_pi complete
+        for (int s = rg * wpc + wid; s < nslab; s += rgs * wpc) {
+          const int i0 = s * 8, ia = i0 + qr;  // this lane's row in the A and C fragments
+          const bool pslab = i0 >= k0 && i0 < k0 + GJB;  // k0 and i0 are multiples of 8: a slab is all pivot rows or none
+          double a[GJB / 4];  // X[ia][4 ks + qc]
 #pragma unroll
-        for (int m = 0; m < GJB; m++) fn[m] = (i < nC && m < kb) ? __ldcg(src + (size_t)i * nC + k0 + m) : 0.0;
-        __syncthreads();
-        for (; i < nC && !gj_bad; i += rstep) {
-          const bool ib = i >= k0 && i < k0 + kb;
-          double g[GJB];  // row coefficients: pivot row -> -P^-1[i-k0][:], other rows -> src[i][pivots] * P^-1
-#pragma unroll
-          for (int l = 0; l < GJB; l++) g[l] = 0.0;
-          if (ib) {
-#pragma unroll
-            for (int l = 0; l < GJB; l++) g[l] = -gj_pi[(i - k0) * GJB + l];
-          } else {
-#pragma unroll
-            for (int m = 0; m < GJB; m++) {
-#pragma unroll
-              for (int l = 0; l < GJB; l++) g[l] += fn[m] * gj_pi[m * GJB + l];
-            }
+          for (int ks = 0; ks < GJB / 4; ks++) {
+            const int m = 4 * ks + qc;
+            a[ks] = pslab ? (ia - k0 == m ? 1.0 : 0.0) : (ia < nC && m < kb) ? -__ldcg(src + (size_t)ia * nC + k0 + m) : 0.0;
           }
-          {
-            const int in = i + rstep;
+          double h[GJB / 8][2];  // H = X P^-1, C layout
 #pragma unroll
-            for (int m = 0; m < GJB; m++) fn[m] = (in < nC && m < kb) ? __ldcg(src + (size_t)in * nC + k0 + m) : 0.0;
+          for (int nt = 0; nt < GJB / 8; nt++) h[nt][0] = h[nt][1] = 0.0;
+#pragma unroll
+          for (int ks = 0; ks < GJB / 4; ks++)
+#pragma unroll
+            for (int nt = 0; nt < GJB / 8; nt++) dmma_884(h[nt][0], h[nt][1], a[ks], gj_pi[(4 * ks + qc) * GJ_LDP + 8 * nt + qr]);
+          // C layout -> A layout: A[qr][4 ks + qc] sits in lane (qr, (4 (ks & 1) + qc) / 2), element qc & 1 of tile ks / 2
+#pragma unroll
+          for (int ks = 0; ks < GJB / 4; ks++) {
+            const int sl = (lane & ~3) | ((4 * (ks & 1) + qc) >> 1);
+            const double v0 = __shfl_sync(0xffffffffu, h[ks >> 1][0], sl);
+            const double v1 = __shfl_sync(0xffffffffu, h[ks >> 1][1], sl);
+            a[ks] = (qc & 1) ? v1 : v0;
           }
+          const bool rowok = ia < nC;
+          const double* srow = src + (size_t)ia * nC;
+          double* drow = dst + (size_t)ia * nC;
+          constexpr int NT = 4;  // column tiles in flight: independent accumulator chains, their base loads issued together
+          for (int n0 = 0; n0 < GJ_CW / 8 && c0 + 8 * n0 < nC; n0 += NT) {
+            double d[NT][2];
 #pragma unroll
-          for (int t = 0; t < GJ_CW / 32; t++) {
-            const int jl = lane + 32 * t, j = c0 + jl;
-            if (j >= nC) break;
-            double v;
-            if (j >= k0 && j < k0 + kb) {
-              const int jj = j - k0;
-              v = 0.0;
+            for (int w = 0; w < NT; w++) {
+              const int j = c0 + 8 * (n0 + w) + 2 * qc;
 #pragma unroll
-              for (int l = 0; l < GJB; l++) v = (l == jj) ? -g[l] : v;
-            } else {
-              v = ib ? 0.0 : __ldcg(src + (size_t)i * nC + j);
-#pragma unroll
-              for (int l = 0; l < GJB; l++) v -= g[l] * gj_rows[l * GJ_CW + jl];
+              for (int x = 0; x < 2; x++) {
+                const int jx = j + x;
+                d[w][x] = (!pslab && rowok && jx < nC && !(jx >= k0 && jx < k0 + kb)) ? __ldcg(srow + jx) : 0.0;
+              }
             }
-            dst[(size_t)i * nC + j] = v;
+#pragma unroll
+            for (int ks = 0; ks < GJB / 4; ks++)
+#pragma unroll
+              for (int w = 0; w < NT; w++)
+                dmma_884(d[w][0], d[w][1], a[ks], gj_rows[(4 * ks + qc) * GJ_LDR + 8 * (n0 + w) + qr]);
+            if (rowok) {
+#pragma unroll
+              for (int w = 0; w < NT; w++) {
+                const int j = c0 + 8 * (n0 + w) + 2 * qc;
+                if (j < nC) drow[j] = d[w][0];
+                if (j + 1 < nC) drow[j + 1] = d[w][1];
+              }
+            }
           }
         }
         __syncthreads();  // readers of gj_rows are done before the next item restages it
       }
-      __syncthreads();
-      if (gj_bad) { bad = true; break; }  // uniform over the grid: every CTA inverted the same pivot block
       grid_barrier(A.bar, target);
     }
     if (bad) coarse = false;
-    Ainv = (((nC + GJB - 1) / GJB) & 1) ? A1 : A0;
+    Ainv = coarse_inverse(A.Ac, nC);
   }
 
   // z = Minv r for the rows of this warp; with the coarse level: += (P yc)[row]

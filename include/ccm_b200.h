@@ -176,6 +176,10 @@ int ccm_ba_debug_schur_blocks(ccm_ba_handle* h, int32_t* rowptr /*K+1*/, int32_t
 /* the PCG path the handle runs: out[0] implementation (1 k_pcg, 2 k_pcg2), out[1] k_pcg CTA size, out[2] coarse aggregate size,
  * out[3] coarse nodes (0: no coarse space) */
 int ccm_ba_debug_paths(ccm_ba_handle* h, int32_t* out /*4*/);
+/* the coarse level of the PCG preconditioner on the S the last ccm_ba_debug_schur left: the assembled Galerkin matrix P^T S P and
+ * its inverse as the PCG set-up computes it (nC = 6 * coarse nodes, row-major nC x nC each).  Fails when the handle has no
+ * coarse space or the set-up meets a non-positive pivot. */
+int ccm_ba_debug_coarse(ccm_ba_handle* h, double* Ac /*nC*nC*/, double* Ainv /*nC*nC*/);
 /* time `reps` launches of one kernel with CUDA events on the handle's stream; returns mean ms per launch.
  * which: 0 linearize (landmark pass, Hll/bl and Z), 1 pose pass, 2 residual/chi2, 3 Z-only linearize (g and Z at lambda),
  * 4 schur products, 5 back-substitution */
