@@ -561,6 +561,48 @@ def distinctive_descriptors(sc, host=False):
     _chk(fn(K, _p(a["bad"]), P, _p(a["ptr"]), _p(a["obs"]), _p(a["desc"]), _p(out["best"]), _p(out["best_median"]), _p(out["desc"])))
     return out
 
+
+def covisibility_batch(sc, batch=None):
+    """The batch arrays of ccm_covisibility for the keyframe rows `batch` (None: sc["batch"]) of a scene as synth.make_covisibility
+    builds it: batch (B,) i32, kf_mp_ptr (B+1,) i64, kf_mp i32 (each row's mvpMapPoints in index order, -1 null)."""
+    batch = np.ascontiguousarray(sc["batch"] if batch is None else batch, np.int32)
+    mptr = np.asarray(sc["mvp_ptr"], np.int64)
+    n = mptr[batch + 1] - mptr[batch]
+    ptr = np.zeros(len(batch) + 1, np.int64); ptr[1:] = np.cumsum(n)
+    idx = np.repeat(mptr[batch] - ptr[:-1], n) + np.arange(ptr[-1])
+    return batch, ptr, np.ascontiguousarray(np.asarray(sc["mvp"], np.int32)[idx])
+
+
+def covisibility(sc, th=15, host=False, capacity=None, batch=None):
+    """KeyFrame::UpdateConnections' weights and ordered connections (cslam/src/KeyFrame.cpp:629-711) for a batch of keyframes, see
+    include/ccm_b200.h.  sc: dict(kf_id (K,) u64, kf_rank (K,) u32, mvp_ptr (K+1,) i64, mvp, mp_bad (P,) u8, obs_ptr (P+1,) i64, obs_kf,
+    batch), as synth.make_covisibility builds it.  Returns dict(conn_ptr (B+1,) i64, conn_kf, conn_w: KFcounter by ascending rank;
+    n_sel (B,), sel_kf, sel_w: the ordered selection in the first n_sel slots of each range; status (B,) u8).  host=False:
+    ccm_covisibility on the GPU; host=True: ccm_covisibility_host.  capacity None: a guess, then the exact total if refused."""
+    b, mptr, mp = covisibility_batch(sc, batch)
+    B = len(b)
+    a = [np.ascontiguousarray(sc[k], t) for k, t in (("kf_id", np.uint64), ("kf_rank", np.uint32), ("mp_bad", np.uint8),
+                                                     ("obs_ptr", np.int64), ("obs_kf", np.int32))]
+    fn = lib().ccm_covisibility_host if host else lib().ccm_covisibility
+    total = np.zeros(1, np.int64)
+    cap = int(capacity) if capacity is not None else min(int(mptr[-1]) * 32, 64 * B + 4096)
+    while True:
+        out = dict(conn_ptr=np.zeros(B + 1, np.int64), conn_kf=np.zeros(max(cap, 1), np.int32), conn_w=np.zeros(max(cap, 1), np.int32),
+                   n_sel=np.zeros(B, np.int32), sel_kf=np.zeros(max(cap, 1), np.int32), sel_w=np.zeros(max(cap, 1), np.int32),
+                   status=np.zeros(B, np.uint8))
+        rc = fn(len(a[0]), _p(a[0]), _p(a[1]), B, _p(b), _p(mptr), _p(mp), len(a[2]), _p(a[2]), _p(a[3]), _p(a[4]), int(th), C.c_int64(cap),
+                _p(out["conn_ptr"]), _p(out["conn_kf"]), _p(out["conn_w"]), _p(out["n_sel"]), _p(out["sel_kf"]), _p(out["sel_w"]),
+                _p(out["status"]), _p(total))
+        if rc != 0 and capacity is None and total[0] > cap:
+            cap = int(total[0])
+            continue
+        _chk(rc)
+        break
+    T = int(total[0])
+    for k in ("conn_kf", "conn_w", "sel_kf", "sel_w"):
+        out[k] = out[k][:T]
+    return out
+
 class MapMirror:
     """Persistent flat mirror of the map for the global BA (ccm_mirror_*, include/ccm_b200.h; SURVEY.md §8(f) rank 1): told about
     changes as they happen, hands out the ccm_ba_problem MapFusionGBA's flattening (S/Optimizer.cpp:658-787) would build."""

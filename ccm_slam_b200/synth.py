@@ -566,3 +566,83 @@ def make_distinctive(p: BAProblem | None = None, seed=0, K=60, P=2000, max_deg=8
     kf_uid = (np.uint64(3) << np.uint64(40)) + np.arange(K, dtype=np.uint64) * np.uint64(7) + np.uint64(11)
     return dict(kf_bad=kf_bad, kf_uid=kf_uid, kf_nfeat=nfeat.astype(np.int32), kf_desc_ptr=kptr, kf_desc=kf_desc, obs_ptr=ptr,
                 obs_kf=obs_kf.astype(np.int32), obs_feat=obs_feat.astype(np.int32), obs_desc=obs_desc, mp_bad=mp_bad)
+
+
+def covis_pack(K, pair_kf, pair_mp, P, rng, kf_id=None, kf_rank=None, null_frac=0.0, dup_frac=0.0, bad_mp_frac=0.0, bad_kf_frac=0.0,
+               extra=None, batch=None):
+    """The arrays of a covisibility scene (synth.make_covisibility) from (keyframe, point) observation pairs, made unique.  Each
+    keyframe's mvpMapPoints holds its points at shuffled indices, with null_frac nulls and dup_frac of its points at a second index;
+    extra: (kf, mp) entries appended to mvpMapPoints without an observation (a point the keyframe lists but that does not list it)."""
+    key = np.unique(np.asarray(pair_kf, np.int64) * max(P, 1) + np.asarray(pair_mp, np.int64))
+    pk, pm = key // max(P, 1), key % max(P, 1)
+    kf_id = np.arange(K, dtype=np.uint64) if kf_id is None else np.asarray(kf_id, np.uint64)
+    kf_rank = rng.permutation(K).astype(np.uint32) if kf_rank is None else np.asarray(kf_rank, np.uint32)
+    ek, em = [pk], [pm]
+    if null_frac > 0:
+        n = rng.binomial(np.bincount(pk, minlength=K), null_frac)
+        ek.append(np.repeat(np.arange(K), n)); em.append(np.full(int(n.sum()), -1, np.int64))
+    if dup_frac > 0:
+        d = np.flatnonzero(rng.random(len(pk)) < dup_frac)
+        ek.append(pk[d]); em.append(pm[d])
+    if extra is not None:
+        ek.append(np.asarray(extra[0], np.int64)); em.append(np.asarray(extra[1], np.int64))
+    ek, em = np.concatenate(ek), np.concatenate(em)
+    o = np.lexsort((rng.random(len(ek)), ek))
+    ek, em = ek[o], em[o]
+    mvp_ptr = np.zeros(K + 1, np.int64); mvp_ptr[1:] = np.cumsum(np.bincount(ek, minlength=K))
+    # observers of each point in ascending rank (std::map<kfptr,size_t>'s order), idx = the point's first index in the keyframe
+    o = np.lexsort((kf_rank[pk], pm))
+    obs_mp, obs_kf = pm[o], pk[o]
+    obs_ptr = np.zeros(P + 1, np.int64); obs_ptr[1:] = np.cumsum(np.bincount(obs_mp, minlength=P))
+    pos = np.arange(len(ek)) - mvp_ptr[ek]
+    live = em >= 0
+    ekey = ek[live] * max(P, 1) + em[live]
+    first = np.lexsort((pos[live], ekey))
+    ukey, at = np.unique(ekey[first], return_index=True)
+    okey = obs_kf * max(P, 1) + obs_mp
+    obs_idx = pos[live][first][at][np.searchsorted(ukey, okey)] if len(okey) else np.zeros(0, np.int64)
+    return dict(kf_id=kf_id, kf_rank=kf_rank, kf_bad=(rng.random(K) < bad_kf_frac).astype(np.uint8), mvp_ptr=mvp_ptr,
+                mvp=em.astype(np.int32), mp_bad=(rng.random(P) < bad_mp_frac).astype(np.uint8), obs_ptr=obs_ptr,
+                obs_kf=obs_kf.astype(np.int32), obs_idx=obs_idx.astype(np.int32),
+                batch=np.arange(K, dtype=np.int32) if batch is None else np.asarray(batch, np.int32))
+
+
+def make_covisibility(p: BAProblem | None = None, seed=0, K=60, P=2000, max_deg=8, window=None, n_maps=1, null_frac=0.05, dup_frac=0.01,
+                      bad_mp_frac=0.03, bad_kf_frac=0.05, same_id_frac=0.0, hub=0, batch_frac=1.0):
+    """Inputs of ccm_covisibility (KeyFrame::UpdateConnections over a batch, include/ccm_b200.h) for the observation lists of a BA
+    problem `p` (None: K keyframes and P points, 1..max_deg observers each, drawn from a window of `window` consecutive rows when
+    given, so that weights spread around the threshold).  Keyframe ids: n_maps maps of consecutive rows, mId = (index in its map, map)
+    packed as map << 32 | index; same_id_frac of the rows take the mId of another row of their map (the self test compares mId, not
+    the row).  Address ranks are a random permutation.  hub > 0: row 0 is co-observed with every one of `hub` other keyframes
+    (K grows to hub + 1 if needed) through extra points, two to six observers each.  batch_frac < 1: a random subset of rows.
+    Returns kf_id (u64), kf_rank (u32), kf_bad, mvp_ptr (K+1), mvp (-1 null), mp_bad, obs_ptr, obs_kf, obs_idx, batch."""
+    rng = np.random.default_rng(seed)
+    if p is None:
+        if hub:
+            K = max(K, hub + 1)
+        deg = rng.integers(1, max_deg + 1, P)
+        mp = np.repeat(np.arange(P, dtype=np.int64), deg)
+        if window:
+            start = rng.integers(0, max(K - window, 1), P)
+            kf = np.repeat(start, deg) + rng.integers(0, min(window, K), len(mp))
+        else:
+            kf = rng.integers(0, K, len(mp))
+    else:
+        K, P = p.K, p.P
+        kf, mp = p.obs_kf.astype(np.int64), p.obs_mp.astype(np.int64)
+    if hub:
+        n_hub = (hub + 1) // 2
+        hp = P + np.arange(n_hub)
+        others = 1 + (np.arange(2 * n_hub) % hub)
+        extra_n = rng.integers(0, 5, n_hub)
+        kf = np.concatenate([kf, np.zeros(n_hub, np.int64), others, rng.integers(1, K, int(extra_n.sum()))])
+        mp = np.concatenate([mp, hp, np.repeat(hp, 2), np.repeat(hp, extra_n)])
+        P += n_hub
+    per_map = -(-K // n_maps)
+    m, first = np.arange(K) // per_map, np.arange(K) % per_map
+    same = np.flatnonzero((rng.random(K) < same_id_frac) & (first > 1))
+    first[same] = first[same] - 1                                       # the mId of the row before it
+    kf_id = (m.astype(np.uint64) << np.uint64(32)) | first.astype(np.uint64)
+    batch = np.arange(K) if batch_frac >= 1 else np.sort(rng.choice(K, max(1, int(K * batch_frac)), replace=False))
+    return covis_pack(K, kf, mp, P, rng, kf_id=kf_id, null_frac=null_frac, dup_frac=dup_frac, bad_mp_frac=bad_mp_frac,
+                      bad_kf_frac=bad_kf_frac, batch=batch)

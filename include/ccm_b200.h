@@ -708,6 +708,40 @@ int ccm_kfstore_distinctive_descriptors(ccm_kf_store* store, int32_t n_kf, const
                                         const int64_t* obs_ptr, const int32_t* obs_kf, const int32_t* obs_feat, int32_t* best,
                                         int32_t* best_median, uint8_t* desc_out);
 
+/* ---- covisibility weights --------------------------------------------------------------------------------------------
+ * The counting and the two orders of KeyFrame::UpdateConnections (cslam/src/KeyFrame.cpp:629-711) for a batch of keyframes, exactly
+ * (integer work).  For batch keyframe b (row batch[b]): every entry of its mvpMapPoints that is not null and whose point is not bad
+ * (a point at two indices counts twice) adds 1 to the weight of each of the point's observers whose kf_id differs from its own (the
+ * idpair, not the row: another row with the same mId is skipped too; bad observers are counted).
+ *   kf_id [n_kf]          mId of each keyframe row, packed (any injective packing of the idpair)
+ *   kf_rank [n_kf]        each row's place in std::map<kfptr,int>'s order (the address rank); a permutation of 0 .. n_kf-1
+ *   batch [n_b]           the keyframe row of each batch entry
+ *   kf_mp_ptr [n_b+1], kf_mp [kf_mp_ptr[n_b]]   entry b's mvpMapPoints in index order as point rows, -1 = null
+ *   mp_bad [n_mp]         isBad() of each point
+ *   obs_ptr [n_mp+1], obs_kf [obs_ptr[n_mp]]    the observers of each point (its GetObservations() keys); observers may lie
+ *                         outside the batch
+ *   th                    the threshold (15 in the reference)
+ * Out, for entry b at conn_ptr[b] .. conn_ptr[b+1) of arrays of `capacity` elements:
+ *   conn_kf / conn_w      KFcounter (mConnectedKeyFrameWeights): (row, weight), ascending rank
+ *   sel_kf / sel_w        the first n_sel[b] slots: the ordered connections (mvpOrderedConnectedKeyFrames / mvOrderedWeights as
+ *                         UpdateConnections writes them): every entry with weight >= th by weight descending, ties by rank
+ *                         descending; when none reaches th, the single entry (nmax, pKFmax), the LOWEST-rank entry among the tied
+ *                         maxima.  The slots after n_sel[b] read -1 / 0.
+ *   status [n_b]          0: the counter is empty (the reference returns with nothing changed), 1 otherwise
+ *   total                 conn_ptr[n_b], always written.  When capacity is below it the call fails with CCM_ERR_INVALID and no
+ *                         other output is written.
+ * A row out of range (batch, point or observer) fails with CCM_ERR_INVALID and a message naming the batch keyframe; nothing is written.
+ * ccm_covisibility runs on the GPU (host buffers in and out, its own stream); ccm_covisibility_host is the same contract on the host,
+ * usable without a device, for the keyframes that ingest connects one at a time. */
+int ccm_covisibility(int32_t n_kf, const uint64_t* kf_id, const uint32_t* kf_rank, int32_t n_b, const int32_t* batch, const int64_t* kf_mp_ptr,
+                     const int32_t* kf_mp, int32_t n_mp, const uint8_t* mp_bad, const int64_t* obs_ptr, const int32_t* obs_kf, int32_t th,
+                     int64_t capacity, int64_t* conn_ptr, int32_t* conn_kf, int32_t* conn_w, int32_t* n_sel, int32_t* sel_kf, int32_t* sel_w,
+                     uint8_t* status, int64_t* total);
+int ccm_covisibility_host(int32_t n_kf, const uint64_t* kf_id, const uint32_t* kf_rank, int32_t n_b, const int32_t* batch,
+                          const int64_t* kf_mp_ptr, const int32_t* kf_mp, int32_t n_mp, const uint8_t* mp_bad, const int64_t* obs_ptr,
+                          const int32_t* obs_kf, int32_t th, int64_t capacity, int64_t* conn_ptr, int32_t* conn_kf, int32_t* conn_w,
+                          int32_t* n_sel, int32_t* sel_kf, int32_t* sel_w, uint8_t* status, int64_t* total);
+
 #ifdef __cplusplus
 }
 #endif
