@@ -603,6 +603,74 @@ def covisibility(sc, th=15, host=False, capacity=None, batch=None):
         out[k] = out[k][:T]
     return out
 
+class NewPtsViewC(C.Structure):
+    _fields_ = [("v", TriViewC), ("Tcw", C.c_float * 12), ("Ow", C.c_float * 3), ("level_sigma2", C.c_void_p),
+                ("scale_factors", C.c_void_p), ("nlevels", C.c_int32), ("scale_factor", C.c_float)]
+
+
+class NewPtsNeighbourC(C.Structure):
+    _fields_ = [("view", NewPtsViewC), ("F12", C.c_float * 9), ("ex", C.c_float), ("ey", C.c_float)]
+
+
+NEW_POINT_DTYPE = np.dtype([("nb", np.int32), ("idx1", np.int32), ("idx2", np.int32), ("x3D", np.float32, 3)])
+NEWPTS_VERDICTS = ("none", "accepted", "parallax", "w_zero", "depth1", "depth2", "reproj1", "reproj2", "dist_zero", "scale", "claimed")
+
+
+def new_points_structs(cur, neighbours, keep):
+    """The C structs of ccm_new_map_points for view dicts as synth_match.make_new_points_scene builds them; `keep` collects what
+    must outlive the call.  A view: desc (n,32) u8, has_mp, kp_xy (n,2), octave, angle, node (n,) vocabulary node of each feature,
+    intr (fx, fy, cx, cy), Tcw (3,4), Ow, level_sigma2, scale_factors, scale_factor; a neighbour adds F12 (3,3), ex, ey."""
+    def view(v):
+        n = len(v["octave"])
+        a = dict(desc=np.ascontiguousarray(v["desc"], np.uint8), has=np.ascontiguousarray(v["has_mp"], np.uint8),
+                 xy=np.ascontiguousarray(v["kp_xy"], np.float32), oc=np.ascontiguousarray(v["octave"], np.int32),
+                 an=np.ascontiguousarray(v["angle"], np.float32), ls=np.ascontiguousarray(v["level_sigma2"], np.float32),
+                 sf=np.ascontiguousarray(v["scale_factors"], np.float32))
+        node = np.asarray(v["node"])
+        ids, counts = np.unique(node, return_counts=True)
+        a["node_id"] = ids.astype(np.uint32)
+        a["node_ptr"] = np.concatenate([[0], np.cumsum(counts)]).astype(np.int32)
+        a["feat"] = np.argsort(node, kind="stable").astype(np.uint32)
+        for k in ("node_id", "node_ptr", "feat"):          # a test may hand in a malformed FeatureVector
+            if "fv_" + k in v:
+                a[k] = np.ascontiguousarray(v["fv_" + k], a[k].dtype)
+        fv = FeatureVectorC(len(a["node_id"]), _p(a["node_id"]), _p(a["node_ptr"]), _p(a["feat"]))
+        keep.extend([a, fv])
+        fx, fy, cx, cy = (float(x) for x in v["intr"])
+        tv = TriViewC(_p(a["desc"]), n, _p(a["has"]), _p(a["xy"]), _p(a["oc"]), _p(a["an"]), C.pointer(fv), fx, fy, cx, cy)
+        T = (C.c_float * 12)(*np.asarray(v["Tcw"], np.float32).reshape(12))
+        O = (C.c_float * 3)(*np.asarray(v["Ow"], np.float32).reshape(3))
+        return NewPtsViewC(tv, T, O, _p(a["ls"]), _p(a["sf"]), len(a["ls"]), float(v["scale_factor"]))
+    c = view(cur)
+    nbs = (NewPtsNeighbourC * max(len(neighbours), 1))()
+    for i, v in enumerate(neighbours):
+        nbs[i] = NewPtsNeighbourC(view(v), (C.c_float * 9)(*np.asarray(v["F12"], np.float32).reshape(9)), float(v["ex"]), float(v["ey"]))
+    return c, nbs
+
+
+def new_map_points(cur, neighbours, want_debug=False, host=False, capacity=None, fn=None):
+    """LocalMapping::CreateNewMapPoints (cslam/src/Mapping.cpp:284-469) for `cur` and all `neighbours` in one call, see
+    include/ccm_b200.h.  Returns the new points as a structured array (nb, idx1, idx2, x3D) in the reference's creation order; with
+    want_debug also best2 and verdict, each (len(neighbours), n).  host=False: ccm_new_map_points on the GPU; host=True:
+    ccm_new_map_points_host.  capacity None: room for every (neighbour, feature) pair."""
+    keep = []
+    c, nbs = new_points_structs(cur, neighbours, keep)
+    n, B = len(cur["octave"]), len(neighbours)
+    cap = n * B if capacity is None else int(capacity)
+    out = np.zeros(max(cap, 1), NEW_POINT_DTYPE)
+    n_out = C.c_int32(-1)
+    best2 = np.full((B, n), -2, np.int32) if want_debug else None
+    verdict = np.full((B, n), 255, np.uint8) if want_debug else None
+    fn = fn or (lib().ccm_new_map_points_host if host else lib().ccm_new_map_points)
+    rc = fn(C.byref(c), nbs, B, _p(out), cap, C.byref(n_out), _p(best2), _p(verdict))
+    if rc != 0:
+        e = CCMError(rc, lib().ccm_last_error().decode())
+        e.needed = n_out.value
+        raise e
+    pts = out[:n_out.value].copy()
+    return (pts, best2, verdict) if want_debug else pts
+
+
 class MapMirror:
     """Persistent flat mirror of the map for the global BA (ccm_mirror_*, include/ccm_b200.h; SURVEY.md §8(f) rank 1): told about
     changes as they happen, hands out the ccm_ba_problem MapFusionGBA's flattening (S/Optimizer.cpp:658-787) would build."""

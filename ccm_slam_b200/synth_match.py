@@ -207,3 +207,164 @@ def place_db_bow(db, k):
 
 def place_db_covis(db, k):
     return db["covis_uid"][db["covis_ptr"][k]:db["covis_ptr"][k + 1]]
+
+
+# ---- a keyframe and its covisible neighbours for LocalMapping::CreateNewMapPoints ------------------------------------------------
+def _rot(rv):
+    th = np.linalg.norm(rv)
+    if th < 1e-12:
+        return np.eye(3)
+    k = rv / th
+    K = np.array([[0, -k[2], k[1]], [k[2], 0, -k[0]], [-k[1], k[0], 0]])
+    return np.eye(3) + np.sin(th) * K + (1 - np.cos(th)) * (K @ K)
+
+
+def new_points_prelude(cur, v):
+    """F12 and the epipole of neighbour `v` against `cur`, in f32, the way ComputeF12 (cslam/src/Mapping.cpp:549-566) and
+    SearchForTriangulation's head (cslam/src/ORBmatcher.cpp:707-714) form them."""
+    f = np.float32
+    R1w, t1w = cur["Tcw"][:, :3].astype(f), cur["Tcw"][:, 3].astype(f)
+    R2w, t2w = v["Tcw"][:, :3].astype(f), v["Tcw"][:, 3].astype(f)
+    R12 = (R1w @ R2w.T).astype(f)
+    t12 = (-(R1w @ R2w.T) @ t2w + t1w).astype(f)
+    tx = np.array([[0, -t12[2], t12[1]], [t12[2], 0, -t12[0]], [-t12[1], t12[0], 0]], f)
+
+    def K(i):
+        fx, fy, cx, cy = i
+        return np.array([[fx, 0, cx], [0, fy, cy], [0, 0, 1]], f)
+    F12 = (np.linalg.inv(K(cur["intr"]).T).astype(f) @ tx @ R12 @ np.linalg.inv(K(v["intr"])).astype(f)).astype(f)
+    C2 = (R2w @ cur["Ow"].astype(f) + t2w).astype(f)
+    with np.errstate(divide="ignore", invalid="ignore", over="ignore"):
+        invz = f(1.0) / C2[2]
+        ex = f(v["intr"][0]) * C2[0] * invz + f(v["intr"][2])
+        ey = f(v["intr"][1]) * C2[1] * invz + f(v["intr"][3])
+    return F12, f(ex), f(ey)
+
+
+def make_new_points_scene(n_nb=20, n=1000, seed=0, n_nodes=None, has_mp_frac=0.4, noise_px=0.4, outlier_frac=0.04, outlier_px=5.0,
+                          octave_jump_frac=0.05, cross_frac=0.05, forward_every=5, decoy_frac=0.06, twin_frac=0.03, tie_frac=0.03, zero_baseline_nb=None, no_shared_nb=None,
+                          all_have_mp=False):
+    """A current keyframe and `n_nb` neighbours looking at one seeded point cloud.  Poses have a real baseline; mvKeysUn are projections
+    plus pixel noise; octaves follow depth (so the scale gate passes for true matches); descriptors are a per-point base with bits
+    flipped per observation; a feature's vocabulary node follows its point.  What forces each outcome to occur:
+      zero_baseline_nb   that neighbour sits 1 mm from the current keyframe: every pair fails the parallax gate
+      outlier_frac       pixels displaced by outlier_px
+      cross_frac         neighbour features moved 3 to 6.5 px off the epipolar line and put on the coarsest level, where the line gate
+                         is wide, against a fine-level feature of the current keyframe: the reprojection gates
+      forward_every      every such neighbour moves along the optical axis, so the epipole lies in the image and decoys fall on both
+                         sides of it: points in front of one camera and behind the other
+      octave_jump_frac   neighbour octaves moved by four levels: the scale gate
+      decoy_frac         copies of a current feature's descriptor placed along its epipolar line in the neighbour: points behind a
+                         camera, low parallax, wrong scale
+      has_mp_frac        features already carrying map points, in either view
+      twin_frac          a second feature of the current keyframe on the same point: two idx1 sharing one idx2
+      tie_frac           a second, identical feature in the neighbour a quarter pixel away: equal distances inside a node
+      no_shared_nb       that neighbour's node ids are disjoint from the current keyframe's
+      all_have_mp        every feature of the current keyframe carries a map point: nothing to search
+    Every neighbour sees most of the cloud, so a feature is matchable in several of them (claims).
+    Returns dict(cur=view, neighbours=[view + F12, ex, ey]); a view is what api.new_map_points reads."""
+    rng = np.random.default_rng(seed)
+    f = np.float32
+    intr = (f(458.654), f(457.296), f(367.215), f(248.375))
+    W, H = 752.0, 480.0
+    P = n
+    n_nodes = n_nodes or max(4, n // 10)
+    X = np.stack([rng.uniform(-5, 5, P), rng.uniform(-3.2, 3.2, P), rng.uniform(4.0, 12.0, P)], 1)
+    base_desc = rng.integers(0, 256, size=(P, 32), dtype=np.uint8)
+    base_oct = rng.integers(0, 4, P)
+    node_of_point = rng.integers(0, n_nodes, P) * 7 + 3
+
+    def make_view(R, t, disjoint=False):
+        Xc = X @ R.T + t
+        z = Xc[:, 2]
+        with np.errstate(divide="ignore", invalid="ignore"):
+            u = intr[0] * Xc[:, 0] / z + intr[2]
+            v = intr[1] * Xc[:, 1] / z + intr[3]
+        vis = np.flatnonzero((z > 0.5) & (u > 0) & (u < W) & (v > 0) & (v < H) & (rng.random(P) < 0.85))
+        vis = rng.permutation(vis)[: n - n // 8]
+        m = len(vis)
+        xy = np.stack([u[vis], v[vis]], 1) + rng.normal(0, noise_px, (m, 2))
+        out = rng.random(m) < outlier_frac
+        xy[out] += rng.normal(0, outlier_px, (int(out.sum()), 2))
+        d = np.linalg.norm(Xc[vis], axis=1)
+        octave = np.clip(np.round(np.log(12.0 / d) / np.log(1.2)).astype(np.int64) + base_oct[vis], 0, 7)
+        desc = flip_bits(base_desc[vis], rng.integers(0, 22, m), rng)
+        node = node_of_point[vis].copy()
+        point = vis.copy()
+        k = n - m                                                   # clutter: features of nothing in the cloud
+        xy = np.concatenate([xy, rng.uniform([0, 0], [W, H], (k, 2))])
+        octave = np.concatenate([octave, rng.integers(0, 8, k)])
+        desc = np.concatenate([desc, rng.integers(0, 256, (k, 32), dtype=np.uint8)])
+        node = np.concatenate([node, rng.integers(0, n_nodes, k) * 7 + 3])
+        point = np.concatenate([point, np.full(k, -1)])
+        if disjoint:
+            node = node + 1
+        Tcw = np.concatenate([R, t[:, None]], 1).astype(f)
+        Ow = (-(Tcw[:, :3].T @ Tcw[:, 3])).astype(f)
+        has = (rng.random(n) < has_mp_frac).astype(np.uint8)
+        return dict(desc=desc, has_mp=has, kp_xy=xy.astype(f), octave=octave.astype(np.int32),
+                    angle=rng.uniform(0, 360, n).astype(f), node=node.astype(np.int64), point=point, intr=intr, Tcw=Tcw, Ow=Ow,
+                    level_sigma2=LEVEL_SIGMA2.copy(), scale_factors=SCALE_FACTORS.copy(), scale_factor=f(1.2), n_seen=m)
+
+    cur = make_view(np.eye(3), np.zeros(3))
+    free = cur["n_seen"]
+    # twins: clutter slots of the current keyframe become second features on points it already sees
+    for s in range(free, min(n, free + int(twin_frac * n))):
+        src = int(rng.integers(0, free))
+        cur["kp_xy"][s] = cur["kp_xy"][src] + f(0.25)
+        cur["octave"][s] = cur["octave"][src]
+        cur["desc"][s] = flip_bits(cur["desc"][src:src + 1], [1], rng)[0]
+        cur["node"][s] = cur["node"][src]; cur["point"][s] = cur["point"][src]; cur["has_mp"][s] = 0; cur["has_mp"][src] = 0
+    if all_have_mp:
+        cur["has_mp"][:] = 1
+    nbs = []
+    for b in range(n_nb):
+        base = 1e-3 if b == zero_baseline_nb else rng.uniform(0.25, 1.1)
+        c = rng.normal(0, 1, 3); c[2] *= 0.4
+        if forward_every and b % forward_every == forward_every - 1:
+            c = np.array([rng.normal(0, 0.08), rng.normal(0, 0.08), rng.choice([-1.0, 1.0])])
+        c = c / np.linalg.norm(c) * base
+        R = _rot(rng.normal(0, 0.04, 3) * (0.0 if b == zero_baseline_nb else 1.0))
+        v = make_view(R, -R @ c, disjoint=(b == no_shared_nb))
+        v.update(dict(zip(("F12", "ex", "ey"), new_points_prelude(cur, v))))
+        m = v["n_seen"]
+        slots = list(range(m, n))
+        jump = rng.random(m) < octave_jump_frac
+        v["octave"][:m][jump] = np.clip(v["octave"][:m][jump] + rng.choice([-4, 4], int(jump.sum())), 0, 7)
+        row = {int(q): i for i, q in enumerate(cur["point"][:free])}
+        for j in np.flatnonzero(rng.random(m) < cross_frac):
+            i = row.get(int(v["point"][j]))
+            if i is None or cur["octave"][i] > 2:
+                continue
+            x1, y1 = cur["kp_xy"][i].astype(np.float64)
+            F = v["F12"].astype(np.float64)
+            la, lb = x1 * F[0, 0] + y1 * F[1, 0] + F[2, 0], x1 * F[0, 1] + y1 * F[1, 1] + F[2, 1]
+            nrm = np.hypot(la, lb)
+            if not nrm > 0:
+                continue
+            v["kp_xy"][j] += (np.array([la, lb]) / nrm * rng.uniform(3.0, 6.5) * rng.choice([-1, 1])).astype(f)
+            v["octave"][j] = 7
+        n_tie, n_decoy = int(tie_frac * n), int(decoy_frac * n)
+        for s in slots[:n_tie]:                                    # an identical feature a quarter pixel away, later in the node
+            src = int(rng.integers(0, m))
+            v["kp_xy"][s] = v["kp_xy"][src] + f(0.25)
+            for k in ("octave", "desc", "node", "point"):
+                v[k][s] = v[k][src]
+            v["has_mp"][s] = v["has_mp"][src] = 0
+        for s in slots[n_tie:n_tie + n_decoy]:                     # a copy of a current feature somewhere on its epipolar line
+            i = int(rng.integers(0, free))
+            x1, y1 = cur["kp_xy"][i].astype(np.float64)
+            F = v["F12"].astype(np.float64)
+            la, lb, lc = x1 * F[0, 0] + y1 * F[1, 0] + F[2, 0], x1 * F[0, 1] + y1 * F[1, 1] + F[2, 1], x1 * F[0, 2] + y1 * F[1, 2] + F[2, 2]
+            if abs(lb) > abs(la):
+                x2 = rng.uniform(0, W); y2 = -(la * x2 + lc) / lb
+            else:
+                y2 = rng.uniform(0, H); x2 = -(lb * y2 + lc) / la
+            if not (np.isfinite(x2) and np.isfinite(y2)):
+                continue
+            v["kp_xy"][s] = (x2, y2)
+            v["desc"][s] = flip_bits(cur["desc"][i:i + 1], [int(rng.integers(0, 4))], rng)[0]
+            v["node"][s] = cur["node"][i] + (1 if b == no_shared_nb else 0)
+            v["octave"][s] = cur["octave"][i]; v["has_mp"][s] = 0; v["point"][s] = -2
+        nbs.append(v)
+    return dict(cur=cur, neighbours=nbs)

@@ -742,6 +742,62 @@ int ccm_covisibility_host(int32_t n_kf, const uint64_t* kf_id, const uint32_t* k
                           const int32_t* obs_kf, int32_t th, int64_t capacity, int64_t* conn_ptr, int32_t* conn_kf, int32_t* conn_w,
                           int32_t* n_sel, int32_t* sel_kf, int32_t* sel_w, uint8_t* status, int64_t* total);
 
+/* ---- new map points ----------------------------------------------------------------------------------------------------
+ * LocalMapping::CreateNewMapPoints (cslam/src/Mapping.cpp:284-469) for the current keyframe and all its neighbours in one call: for
+ * each neighbour, SearchForTriangulation as the member constructs its matcher (ORBmatcher(0.6,false): no rotation histogram), then the
+ * triangulation of every match and its gates (:362-448).  The neighbour list, the short-baseline skip (:320-328), ComputeF12 and the
+ * epipole are f32 cv::Mat prelude and stay with the caller, as for ccm_match_triangulation; a skipped neighbour is not passed.
+ *
+ * The only coupling between neighbours in the reference is that a feature of the current keyframe triangulated with neighbour i
+ * carries a map point when neighbour i+1 is searched.  So the lowest neighbour index whose pair is accepted claims the feature; a
+ * rejected pair claims nothing.  Points leave in the reference's creation order: neighbour ascending, idx1 ascending within one.  Two
+ * idx1 may choose the same idx2 of one neighbour; both points are reported.
+ *
+ * Arithmetic: ccm_slam_b200/csrc/new_points_math.cuh, one source for the device and the host entry point, which agree bit for bit.
+ * cv::SVD::compute has no single bit pattern in the reference (its own Jacobi iteration or LAPACK's sgesdd, by OpenCV build); the
+ * library states one: a one-sided Jacobi iteration in f32 (DESIGN.md §5).
+ *
+ * Every feature index may appear at most once in the current keyframe's FeatureVector (DBoW2 lists each feature under one node).
+ * Out: *n_out points in out[]; when capacity is below the count the call fails with CCM_ERR_INVALID, *n_out holds the count needed
+ * and nothing else is written.  best2 / verdict (each n_nb * cur->v.n, or NULL), for neighbour b and feature i at [b * n + i]:
+ * the neighbour feature SearchForTriangulation pairs with i or -1, and what became of the pair.  A feature claimed by an earlier
+ * neighbour reads -1 / CCM_NEWPTS_CLAIMED.  Invalid input fails with CCM_ERR_INVALID and a message naming the neighbour.
+ * ccm_new_map_points: one upload, three launches whatever n_nb, one download.  ccm_new_map_points_host: the same contract, no device. */
+typedef enum ccm_newpts_verdict {
+  CCM_NEWPTS_NONE = 0,       /* no pair: the feature carries a map point, or no neighbour feature passes the matcher's gates */
+  CCM_NEWPTS_ACCEPTED = 1,
+  CCM_NEWPTS_PARALLAX = 2,   /* cosParallaxRays outside (0, 0.9998) */
+  CCM_NEWPTS_W_ZERO = 3,     /* x3D(3) == 0 */
+  CCM_NEWPTS_DEPTH1 = 4,     /* z1 <= 0 */
+  CCM_NEWPTS_DEPTH2 = 5,     /* z2 <= 0 */
+  CCM_NEWPTS_REPROJ1 = 6,    /* reprojection error in the current keyframe above 5.991 * sigma2 */
+  CCM_NEWPTS_REPROJ2 = 7,    /* ... in the neighbour */
+  CCM_NEWPTS_DIST_ZERO = 8,  /* dist1 == 0 || dist2 == 0 */
+  CCM_NEWPTS_SCALE = 9,      /* scale consistency */
+  CCM_NEWPTS_CLAIMED = 10    /* an earlier neighbour's accepted pair gave the feature its map point */
+} ccm_newpts_verdict;
+
+typedef struct ccm_newpts_view {      /* one keyframe as CreateNewMapPoints reads it */
+  ccm_tri_view v;                     /* descriptors, has_mp, mvKeysUn xy / octave / angle (angle is not read), FeatureVector, fx fy cx cy */
+  float Tcw[12];                      /* [Rcw | tcw], 3x4 row-major f32 */
+  float Ow[3];                        /* GetCameraCenter() */
+  const float* level_sigma2;          /* mvLevelSigma2, nlevels */
+  const float* scale_factors;         /* mvScaleFactors, nlevels */
+  int32_t nlevels;
+  float scale_factor;                 /* mfScaleFactor (read of the current keyframe only) */
+} ccm_newpts_view;
+typedef struct ccm_newpts_neighbour {
+  ccm_newpts_view view;
+  float F12[9];                       /* ComputeF12(current, neighbour), row-major */
+  float ex, ey;                       /* the current keyframe's centre projected into the neighbour (cslam/src/ORBmatcher.cpp:707-714) */
+} ccm_newpts_neighbour;
+typedef struct ccm_new_point { int32_t nb, idx1, idx2; float x3D[3]; } ccm_new_point;
+
+int ccm_new_map_points(const ccm_newpts_view* cur, const ccm_newpts_neighbour* nb, int32_t n_nb, ccm_new_point* out, int32_t capacity,
+                       int32_t* n_out, int32_t* best2, uint8_t* verdict);
+int ccm_new_map_points_host(const ccm_newpts_view* cur, const ccm_newpts_neighbour* nb, int32_t n_nb, ccm_new_point* out, int32_t capacity,
+                            int32_t* n_out, int32_t* best2, uint8_t* verdict);
+
 #ifdef __cplusplus
 }
 #endif
