@@ -846,10 +846,16 @@ void build(ccm_ba_handle* h, const ccm_ba_problem* p) {
   h->pcg_prolong = env_int("CCM_PCG_PROLONG", 1) ? 1 : 0;  // cfg5: 1538 -> 617 PCG iterations per Global BA at 192 coarse nodes
   // PCG iterations per Global BA on cfg5: NC 192 refresh 4: 617, NC 192 refresh 2: 545, NC 256 refresh 2: 400, NC 256 refresh 1: 384,
   // NC 384 refresh 4: 357 (its 2304^2 inverse is the most expensive), NC 128 refresh 1: 1014; refresh 8 (one inverse per BA): 1950
-  pcg_coarse_shape(Kf, env_int("CCM_PCG_NC", Kf >= 4096 ? (h->pcg_prolong ? 256 : 384) : 128), &h->pcg_agg, &h->pcg_nc);
+  // From Kf >= 8192 (cfg5: Kf = 9999) 320 nodes: an iteration of k_pcg2 there costs about 110 us, so the iterations a larger coarse
+  // space saves outweigh its dearer inverse; below that the iterations are cheaper and 256 nodes stay the better trade.
+  pcg_coarse_shape(Kf, env_int("CCM_PCG_NC", Kf >= 4096 ? (h->pcg_prolong ? (Kf >= 8192 ? 320 : 256) : 384) : 128), &h->pcg_agg,
+                   &h->pcg_nc);
   // refresh 1 / 2 / 4 with NC 256: 384 / 400 / 496 iterations per cfg5 Global BA.  An iteration of k_pcg2 costs about 120 us and
   // the set-up launch that rebuilds the 1536^2 inverse 2.0 ms, so one BA takes 173 / 167 / 174 ms; cfg4 (k_pcg, nC = 690) takes
   // 27.3 / 24.5 ms at refresh 1 / 2 (H100 80GB HBM3, 700 W).  Every size rebuilds every 2nd solve.
+  // cfg5, one Global BA (8 LM trials, median of 3; H100 80GB HBM3, 700 W), NC x refresh -> PCG iterations, ms:
+  //   256 / 2: 400, 167.5   320 / 2: 262, 157.1   384 / 2: 212, 160.3
+  //   256 / 1: 384, 172.9   320 / 1: 246, 168.7   384 / 1: 197, 179.9
   h->pcg_refresh = std::max(1, env_int("CCM_PCG_REFRESH", 2));
   {
     const size_t nC = (size_t)6 * h->pcg_nc;
