@@ -671,6 +671,78 @@ def new_map_points(cur, neighbours, want_debug=False, host=False, capacity=None,
     return (pts, best2, verdict) if want_debug else pts
 
 
+class FeatureGridC(C.Structure):
+    _fields_ = [("n", C.c_int32), ("desc", C.c_void_p), ("kp_xy", C.c_void_p), ("octave", C.c_void_p), ("angle", C.c_void_p),
+                ("min_x", C.c_float), ("min_y", C.c_float), ("max_x", C.c_float), ("max_y", C.c_float),
+                ("grid_w_inv", C.c_float), ("grid_h_inv", C.c_float), ("grid_cols", C.c_int32), ("grid_rows", C.c_int32)]
+
+
+def grid_struct(g, keep):
+    """ccm_feature_grid from dict(desc, kp_xy, octave, angle, bounds=(mnMinX, mnMinY, mnMaxX, mnMaxY), cols, rows)"""
+    a = dict(desc=np.ascontiguousarray(g["desc"], np.uint8), xy=np.ascontiguousarray(g["kp_xy"], np.float32),
+             oc=np.ascontiguousarray(g["octave"], np.int32), an=np.ascontiguousarray(g["angle"], np.float32))
+    keep.append(a)
+    x0, y0, x1, y1 = [np.float32(v) for v in g["bounds"]]
+    wi = np.float32(g["cols"]) / np.float32(x1 - x0)   # mfGridElementWidthInv  (S/Frame.cpp:86)
+    hi = np.float32(g["rows"]) / np.float32(y1 - y0)   # mfGridElementHeightInv (S/Frame.cpp:87)
+    return FeatureGridC(a["desc"].shape[0], _p(a["desc"]), _p(a["xy"]), _p(a["oc"]), _p(a["an"]), x0, y0, x1, y1, wi, hi,
+                        int(g["cols"]), int(g["rows"]))
+
+
+class FuseKfC(C.Structure):
+    _fields_ = [("grid", FeatureGridC), ("Tcw", C.c_float * 12), ("Ow", C.c_float * 3), ("fx", C.c_float), ("fy", C.c_float),
+                ("cx", C.c_float), ("cy", C.c_float), ("scale_factors", C.c_void_p), ("inv_level_sigma2", C.c_void_p),
+                ("nlevels", C.c_int32), ("log_scale_factor", C.c_float)]
+
+
+class FusePointsC(C.Structure):
+    _fields_ = [("n", C.c_int32), ("pos", C.c_void_p), ("normal", C.c_void_p), ("max_distance", C.c_void_p),
+                ("min_distance", C.c_void_p), ("desc", C.c_void_p), ("skip", C.c_void_p)]
+
+
+def fuse_structs(sc, keep):
+    """The C structs of ccm_fuse_neighbours for a scene as synth_match.make_fuse_scene builds it; `keep` collects what must outlive
+    the call.  A keyframe: a grid dict (desc, kp_xy, octave, angle, bounds, cols, rows) plus Tcw (3,4), Ow, intr (fx, fy, cx, cy),
+    scale_factors, inv_level_sigma2, log_scale_factor.  sc: cur, targets (distinct keyframes), points dict(pos (P,3), normal (P,3),
+    max_d, min_d, desc (P,32), skip), cur_point (n,) and cand rows."""
+    def kf(k):
+        a = dict(sf=np.ascontiguousarray(k["scale_factors"], np.float32), il=np.ascontiguousarray(k["inv_level_sigma2"], np.float32))
+        keep.append(a)
+        fx, fy, cx, cy = (float(x) for x in k["intr"])
+        return FuseKfC(grid_struct(k, keep), (C.c_float * 12)(*np.asarray(k["Tcw"], np.float32).reshape(12)),
+                       (C.c_float * 3)(*np.asarray(k["Ow"], np.float32).reshape(3)), fx, fy, cx, cy, _p(a["sf"]), _p(a["il"]),
+                       len(a["sf"]), float(k["log_scale_factor"]))
+    cur = kf(sc["cur"])
+    T = len(sc["targets"])
+    tg = (FuseKfC * max(T, 1))()
+    for i, k in enumerate(sc["targets"]):
+        tg[i] = kf(k)
+    p = sc["points"]
+    a = dict(pos=np.ascontiguousarray(p["pos"], np.float32).reshape(-1, 3), nrm=np.ascontiguousarray(p["normal"], np.float32).reshape(-1, 3),
+             mx=np.ascontiguousarray(p["max_d"], np.float32), mn=np.ascontiguousarray(p["min_d"], np.float32),
+             desc=np.ascontiguousarray(p["desc"], np.uint8).reshape(-1, 32), skip=np.ascontiguousarray(p["skip"], np.uint8),
+             cp=np.ascontiguousarray(sc["cur_point"], np.int32), cand=np.ascontiguousarray(sc["cand"], np.int32))
+    keep += [a, tg]
+    pts = FusePointsC(len(a["mx"]), _p(a["pos"]), _p(a["nrm"]), _p(a["mx"]), _p(a["mn"]), _p(a["desc"]), _p(a["skip"]))
+    return cur, tg, T, pts, a["cp"], a["cand"]
+
+
+def fuse_neighbours(sc, host=False, fn=None):
+    """The searches of LocalMapping::SearchInNeighbors (cslam/src/Mapping.cpp:471-547) in one call, see include/ccm_b200.h.
+    Returns (fwd (T, n) i32: keypoint of target t for the current keyframe's slot i or -1; bwd (C,) i32: keypoint of the current
+    keyframe for candidate c or -1; the number of pairs whose PredictScale level was settled with the host's logf).
+    host=False: ccm_fuse_neighbours on the GPU; host=True: ccm_fuse_neighbours_host."""
+    keep = []
+    cur, tg, T, pts, cp, cand = fuse_structs(sc, keep)
+    n = len(cp)
+    fwd = np.full((T, n), -3, np.int32)
+    bwd = np.full(len(cand), -3, np.int32)
+    settled = C.c_int32(-1)
+    fn = fn or (lib().ccm_fuse_neighbours_host if host else lib().ccm_fuse_neighbours)
+    _chk(fn(C.byref(cur), tg, T, C.byref(pts), _p(cp), _p(cand), len(cand), _p(fwd), _p(bwd), C.byref(settled)))
+    return fwd, bwd, settled.value
+
+
 class MapMirror:
     """Persistent flat mirror of the map for the global BA (ccm_mirror_*, include/ccm_b200.h; SURVEY.md §8(f) rank 1): told about
     changes as they happen, hands out the ccm_ba_problem MapFusionGBA's flattening (S/Optimizer.cpp:658-787) would build."""

@@ -84,6 +84,26 @@ struct DevBuf {
 
 inline int div_up(long long a, long long b) { return (int)((a + b - 1) / b); }
 
+// Lays arrays out in one block at 16-byte boundaries, for a single upload (new_points.cu, fuse_neighbours.cu).  Without a host block it
+// only measures; with one it copies each array in and answers the address the array will have on the device.
+struct Packer {
+  size_t at = 0;
+  uint8_t* host = nullptr;
+  const uint8_t* dev = nullptr;
+  size_t reserve(size_t bytes) {
+    const size_t off = at;
+    at = (at + bytes + 15) & ~size_t(15);
+    return off;
+  }
+  template <typename T>
+  const T* put(const T* src, size_t count) {
+    const size_t off = reserve(count * sizeof(T));
+    if (!host) return nullptr;
+    if (count) memcpy(host + off, src, count * sizeof(T));
+    return reinterpret_cast<const T*>(dev + off);
+  }
+};
+
 int current_device();      // device chosen by ccm_init (default 0)
 int sm_count();
 void ensure_device();      // throws CCM_ERR_NO_DEVICE when there is none

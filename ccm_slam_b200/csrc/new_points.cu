@@ -280,26 +280,6 @@ struct Scratch {
 };
 thread_local Scratch t_scr;
 
-// Lays arrays out in one block at 16-byte boundaries.  Without a host block it only measures; with one it copies each array in and
-// answers the address the array will have on the device.
-struct Packer {
-  size_t at = 0;
-  uint8_t* host = nullptr;
-  const uint8_t* dev = nullptr;
-  size_t reserve(size_t bytes) {
-    const size_t off = at;
-    at = (at + bytes + 15) & ~size_t(15);
-    return off;
-  }
-  template <typename T>
-  const T* put(const T* src, size_t count) {
-    const size_t off = reserve(count * sizeof(T));
-    if (!host) return nullptr;
-    if (count) memcpy(host + off, src, count * sizeof(T));
-    return reinterpret_cast<const T*>(dev + off);
-  }
-};
-
 // the View table (views[0] the current keyframe, then the neighbours) followed by every array the views point to
 size_t pack_views(Packer& pk, const ccm_newpts_view* cur, const ccm_newpts_neighbour* nb, int32_t n_nb, const std::vector<int32_t>& ent_node,
                   const std::vector<int32_t>& peer) {

@@ -25,6 +25,58 @@
 
 namespace ccm {
 
+namespace wb {
+CCM_WB_HD unsigned popc(unsigned x) {
+#if defined(__CUDA_ARCH__)
+  return __popc(x);
+#else
+  return (unsigned)__builtin_popcount(x);
+#endif
+}
+// single-rounded f32 operations: no contraction into an FMA on the device, plain operators on the host
+CCM_WB_HD float sub(float a, float b) {
+#if defined(__CUDA_ARCH__)
+  return __fsub_rn(a, b);
+#else
+  return a - b;
+#endif
+}
+CCM_WB_HD float add(float a, float b) {
+#if defined(__CUDA_ARCH__)
+  return __fadd_rn(a, b);
+#else
+  return a + b;
+#endif
+}
+CCM_WB_HD float mul(float a, float b) {
+#if defined(__CUDA_ARCH__)
+  return __fmul_rn(a, b);
+#else
+  return a * b;
+#endif
+}
+}  // namespace wb
+
+// GetFeaturesInArea's cell range (S/KeyFrame.cpp:1170-1184) with its early returns, each operation rounded once: the host grid
+// (CellIndex::range) and the device (fuse_neighbours.cu) use this one copy.  false = no cell.
+CCM_WB_HD bool cell_range(float x, float y, float r, float min_x, float min_y, float w_inv, float h_inv, int cols, int rows, int& c0, int& c1,
+                          int& r0, int& r1) {
+  const float dx = wb::sub(x, min_x), dy = wb::sub(y, min_y);
+  const int a = (int)floorf(wb::mul(wb::sub(dx, r), w_inv));
+  c0 = a > 0 ? a : 0;
+  if (c0 >= cols) return false;
+  const int b = (int)ceilf(wb::mul(wb::add(dx, r), w_inv));
+  c1 = b < cols - 1 ? b : cols - 1;
+  if (c1 < 0) return false;
+  const int c = (int)floorf(wb::mul(wb::sub(dy, r), h_inv));
+  r0 = c > 0 ? c : 0;
+  if (r0 >= rows) return false;
+  const int d = (int)ceilf(wb::mul(wb::add(dy, r), h_inv));
+  r1 = d < rows - 1 ? d : rows - 1;
+  if (r1 < 0) return false;
+  return true;
+}
+
 // mGrid as cell_ptr / cell_feat; cell id = column * rows + row (mGrid[col][row])
 struct CellIndex {
   const ccm_feature_grid& g;
@@ -48,15 +100,7 @@ struct CellIndex {
 
   // GetFeaturesInArea's cell range with its early returns; false = no cell
   bool range(float x, float y, float r, int& c0, int& c1, int& r0, int& r1) const {
-    c0 = std::max(0, (int)floorf((x - g.min_x - r) * g.grid_w_inv));
-    if (c0 >= g.grid_cols) return false;
-    c1 = std::min(g.grid_cols - 1, (int)ceilf((x - g.min_x + r) * g.grid_w_inv));
-    if (c1 < 0) return false;
-    r0 = std::max(0, (int)floorf((y - g.min_y - r) * g.grid_h_inv));
-    if (r0 >= g.grid_rows) return false;
-    r1 = std::min(g.grid_rows - 1, (int)ceilf((y - g.min_y + r) * g.grid_h_inv));
-    if (r1 < 0) return false;
-    return true;
+    return cell_range(x, y, r, g.min_x, g.min_y, g.grid_w_inv, g.grid_h_inv, g.grid_cols, g.grid_rows, c0, c1, r0, r1);
   }
 
   // visits the keypoints GetFeaturesInArea(x, y, r[, lo, hi]) would return, in its order; levels: lo <= octave <= hi
@@ -97,37 +141,6 @@ inline void fill_window_queries(const CellIndex& cells, const ccm_proj_queries& 
   }
 }
 
-namespace wb {
-CCM_WB_HD unsigned popc(unsigned x) {
-#if defined(__CUDA_ARCH__)
-  return __popc(x);
-#else
-  return (unsigned)__builtin_popcount(x);
-#endif
-}
-// single-rounded f32 operations: no contraction into an FMA on the device, plain operators on the host
-CCM_WB_HD float sub(float a, float b) {
-#if defined(__CUDA_ARCH__)
-  return __fsub_rn(a, b);
-#else
-  return a - b;
-#endif
-}
-CCM_WB_HD float add(float a, float b) {
-#if defined(__CUDA_ARCH__)
-  return __fadd_rn(a, b);
-#else
-  return a + b;
-#endif
-}
-CCM_WB_HD float mul(float a, float b) {
-#if defined(__CUDA_ARCH__)
-  return __fmul_rn(a, b);
-#else
-  return a * b;
-#endif
-}
-}  // namespace wb
 
 // One lane's share of one query's window: the cell runs of columns c0..c1 (rows r0..r1) 32 keypoints at a time in visiting
 // order; a keypoint that passes the window / level / chi-square tests forms key = distance << 20 | position-in-visit.  The

@@ -368,3 +368,218 @@ def make_new_points_scene(n_nb=20, n=1000, seed=0, n_nodes=None, has_mp_frac=0.4
             v["octave"][s] = cur["octave"][i]; v["has_mp"][s] = 0; v["point"][s] = -2
         nbs.append(v)
     return dict(cur=cur, neighbours=nbs)
+
+
+# ---- a keyframe and its fuse targets for LocalMapping::SearchInNeighbors --------------------------------------------------------
+def fuse_dist3d(X, Ow):
+    """dist3D of Fuse's prelude: f32 difference, squares summed in f64, rounded to f32"""
+    PO = (np.asarray(X, np.float32) - np.asarray(Ow, np.float32)).astype(np.float64)
+    return np.sqrt((PO * PO).sum(-1)).astype(np.float32)
+
+
+def make_fuse_scene(n_first=20, n_second=5, n=1000, seed=0, dup_frac=0.5, same_frac=0.15, has_mp_frac=0.8, dnr_frac=0.03, bad_frac=0.03,
+                    behind=8, outside=8, off_cone=8, boundary=24, repeat_second=True, third_pairs=40):
+    """A current keyframe, `n_first` first neighbours and up to `n_second` second neighbours each, looking at one seeded point cloud.
+    Every keyframe's features are projections of the cloud plus pixel noise, octaves follow depth, descriptors a per-point base with bits
+    flipped per observation.  The map points (one row each in `points`) and the knobs that force each outcome:
+      dup_frac       a target's feature on a cloud point the current keyframe also holds carries a second point (a duplicate): the
+                     searches pair the two both ways (MapPoint::Replace in the member)
+      same_frac      ... or carries the very point the current slot holds (already in the target: skipped live by the member)
+      has_mp_frac    share of features that carry a point at all
+      dnr_frac       points with mbDoNotReplace; bad_frac  points already bad (skip = 1, kept in the slots)
+      repeat_second  a second neighbour may be listed under several first neighbours (entries repeat a row)
+      behind / outside / off_cone   extra points in the current slots and the candidates: behind the cameras, projecting outside the
+                     image, or with the normal turned away (outside the 60-degree cone)
+      third_pairs    duplicate pairs also observed, at different indices, by a third keyframe that is no target (third_point)
+      boundary       points whose mfMaxDistance / dist3D sits within a few ulps of 1.2^k for the current keyframe (candidates) or for
+                     target 0 (current slots): PredictScale's level hangs on the last bit of logf
+    Returns dict(cur, targets (distinct keyframes), entries (target rows in list order), target_point (per target, the point row of
+    each slot or -1), points, cur_point, cand, conn (ordered connections: [0] the current keyframe's as target rows, [1 + t] target
+    t's, -1 = the current keyframe), third_point, boundary_rows); cand is the first-seen union of the targets' points over entries that are not bad."""
+    rng = np.random.default_rng(seed)
+    f = np.float32
+    intr = (f(458.654), f(457.296), f(367.215), f(248.375))
+    W, H = 752, 480
+    lsf = f(np.log(f(1.2)))
+    P0 = int(n * 1.4)
+    X = np.stack([rng.uniform(-5, 5, P0), rng.uniform(-3.2, 3.2, P0), rng.uniform(4.0, 12.0, P0)], 1).astype(f)
+    base_desc = rng.integers(0, 256, size=(P0, 32), dtype=np.uint8)
+    d_ref = np.linalg.norm(X.astype(np.float64), axis=1)
+    l0 = rng.integers(0, 4, P0)
+    maxd = (d_ref * SCALE_FACTORS[l0]).astype(f)
+    mind = (maxd / SCALE_FACTORS[7]).astype(f)
+    pts = dict(pos=[], normal=[], max_d=[], min_d=[], desc=[], skip=[])
+    dup_of = {}
+
+    def add_point(x, nrm, mx, mn, desc, skip=0):
+        pts["pos"].append(np.asarray(x, f)); pts["normal"].append(np.asarray(nrm, f)); pts["max_d"].append(f(mx)); pts["min_d"].append(f(mn))
+        pts["desc"].append(np.asarray(desc, np.uint8)); pts["skip"].append(int(skip))
+        return len(pts["skip"]) - 1
+
+    def unit(v):
+        v = np.asarray(v, np.float64)
+        return (v / np.linalg.norm(v)).astype(f)
+
+    def make_kf(R, t):
+        Xc = X.astype(np.float64) @ R.T + t
+        z = Xc[:, 2]
+        u = intr[0] * Xc[:, 0] / z + intr[2]
+        v = intr[1] * Xc[:, 1] / z + intr[3]
+        vis = np.flatnonzero((z > 0.5) & (u > 0) & (u < W) & (v > 0) & (v < H) & (rng.random(P0) < 0.85))
+        vis = rng.permutation(vis)[: n - n // 8]
+        m = len(vis)
+        xy = np.stack([u[vis], v[vis]], 1) + rng.normal(0, 0.5, (m, 2))
+        Tcw = np.concatenate([R, t[:, None]], 1).astype(f)
+        Ow = (-(Tcw[:, :3].T @ Tcw[:, 3])).astype(f)
+        dist = fuse_dist3d(X[vis], Ow).astype(np.float64)
+        octave = np.clip(np.ceil(np.log(maxd[vis] / dist) / np.log(1.2)), 0, 7).astype(np.int64)
+        octave = np.where(rng.random(m) < 0.2, np.maximum(octave - 1, 0), octave)
+        desc = flip_bits(base_desc[vis], rng.integers(0, 20, m), rng)
+        k = n - m
+        xy = np.concatenate([xy, rng.uniform([0, 0], [W, H], (k, 2))]).astype(f)
+        octave = np.concatenate([octave, rng.integers(0, 8, k)]).astype(np.int32)
+        desc = np.concatenate([desc, rng.integers(0, 256, (k, 32), dtype=np.uint8)])
+        return dict(desc=desc, kp_xy=xy, octave=octave, angle=np.zeros(n, f), bounds=(0, 0, W, H), cols=64, rows=48, intr=intr, Tcw=Tcw,
+                    Ow=Ow, scale_factors=SCALE_FACTORS.copy(), inv_level_sigma2=INV_LEVEL_SIGMA2.copy(), log_scale_factor=lsf,
+                    world=np.concatenate([vis, np.full(k, -1)]))
+
+    cur = make_kf(np.eye(3), np.zeros(3))
+    n_pool = n_first + max(0, n_second * n_first // 3)
+    targets = []
+    for b in range(n_pool):
+        c = rng.normal(0, 1, 3); c[2] *= 0.4
+        c = c / np.linalg.norm(c) * rng.uniform(0.2, 1.0)
+        R = _rot(rng.normal(0, 0.04, 3))
+        targets.append(make_kf(R, -R @ c))
+    # the current keyframe's points
+    cur_row = {}
+    cur_point = np.full(n, -1, np.int32)
+    for i, w in enumerate(cur["world"]):
+        if w < 0 or rng.random() >= has_mp_frac:
+            continue
+        r = add_point(X[w], unit(X[w] - cur["Ow"]), maxd[w], mind[w], flip_bits(base_desc[w:w + 1], [rng.integers(0, 10)], rng)[0],
+                      rng.random() < dnr_frac + bad_frac)
+        cur_row[int(w)] = r
+        cur_point[i] = r
+    # the targets' points: the current keyframe's own, duplicates of them, or points of their own
+    target_point = []
+    for k in targets:
+        tp = np.full(n, -1, np.int32)
+        for j, w in enumerate(k["world"]):
+            if w < 0 or rng.random() >= has_mp_frac:
+                continue
+            a = rng.random()
+            if int(w) in cur_row and a < same_frac:
+                tp[j] = cur_row[int(w)]
+                continue
+            if int(w) not in cur_row or a < same_frac + dup_frac:
+                xw = X[w] + rng.normal(0, 0.002, 3).astype(f)
+                tp[j] = add_point(xw, unit(xw - k["Ow"]), maxd[w], mind[w], flip_bits(base_desc[w:w + 1], [rng.integers(0, 10)], rng)[0],
+                                  rng.random() < dnr_frac + bad_frac)
+                if int(w) in cur_row:
+                    dup_of[int(tp[j])] = cur_row[int(w)]
+        target_point.append(tp)
+    # the entry list: each first neighbour, then up to n_second second neighbours from the rest of the pool
+    entries, seconds = [], []
+    for b in range(n_first):
+        entries.append(b)
+        pool = np.arange(n_first, n_pool) if n_pool > n_first else np.arange(0)
+        pick = []
+        if len(pool):
+            pick = [int(p) for p in rng.choice(pool, size=min(n_second, len(pool)), replace=False)]
+            if not repeat_second:
+                pick = [p for p in pick if p not in entries]
+            entries.extend(pick)
+        seconds.append(pick)
+    used = sorted(set(entries))
+    remap = {r: i for i, r in enumerate(used)}
+    targets = [targets[r] for r in used]
+    target_point = [target_point[r] for r in used]
+    entries = [remap[r] for r in entries]
+    # each keyframe's ordered connections for the stand-in objects (-1: the current keyframe, which the member skips as a second)
+    conn = [[remap[b] for b in range(n_first)]] + [[] for _ in targets]
+    for b in range(n_first):
+        c = [remap[p] for p in seconds[b]]
+        c.insert(int(rng.integers(0, len(c) + 1)), -1)
+        conn[1 + remap[b]] = c
+    skip = np.asarray(pts["skip"], np.uint8)
+    bad = skip & (rng.random(len(skip)) < bad_frac / max(dnr_frac + bad_frac, 1e-9)).astype(np.uint8)
+    cand, seen = [], set()
+    for e in entries:
+        for r in target_point[e]:
+            if r >= 0 and not bad[r] and r not in seen:
+                seen.add(int(r)); cand.append(int(r))
+    # the knob points, each in a free slot of the current keyframe and at the end of the candidates
+    free = list(np.flatnonzero(cur_point < 0))
+    rng.shuffle(free)
+
+    def knob(x, nrm, mx, mn, desc):
+        r = add_point(x, nrm, mx, mn, desc)
+        if free:
+            cur_point[free.pop()] = r
+        cand.append(r)
+    seen_w = [int(w) for w in cur["world"] if w >= 0]
+    for _ in range(behind):
+        w = seen_w[rng.integers(len(seen_w))]
+        x = X[w] * f(-1.0)
+        knob(x, unit(x), maxd[w], mind[w], base_desc[w])
+    for _ in range(outside):
+        w = seen_w[rng.integers(len(seen_w))]
+        x = X[w] + np.array([rng.choice([-1, 1]) * 40.0, 0, 0], f)
+        knob(x, unit(x), maxd[w] * 4, mind[w], base_desc[w])
+    for _ in range(off_cone):
+        w = seen_w[rng.integers(len(seen_w))]
+        knob(X[w], -unit(X[w]), maxd[w], mind[w], base_desc[w])
+    boundary_rows = []
+    for b in range(boundary):
+        w = seen_w[rng.integers(len(seen_w))]
+        fwd = b % 2 == 0 and len(targets) > 0
+        Ow = targets[0]["Ow"] if fwd else cur["Ow"]
+        d = fuse_dist3d(X[w], Ow)
+        mx = np.float32(np.float64(d) * 1.2 ** int(rng.integers(1, 5)))
+        off = int(rng.integers(0, 9)) - 4                           # a few ulps either side of the boundary
+        for _ in range(abs(off)):
+            mx = np.nextafter(mx, np.float32(np.inf if off > 0 else -np.inf), dtype=np.float32)
+        r = add_point(X[w], unit(X[w] - Ow), mx, mx / SCALE_FACTORS[7], base_desc[w])
+        boundary_rows.append(r)
+        if fwd:
+            if free:
+                cur_point[free.pop()] = r
+        else:
+            cand.append(r)
+    points = {k: np.asarray(v) for k, v in pts.items()}
+    points["skip"] = points["skip"].astype(np.uint8)
+    points["bad"] = np.zeros(len(points["skip"]), np.uint8); points["bad"][:len(bad)] = bad
+    # a third keyframe observing duplicate pairs (a current point and its duplicate in a target) at different indices: Replace's
+    # id-mismatch branch when the pair fuses
+    pairs = [(a, b) for b, a in dup_of.items() if cur_point.tolist().count(a) == 1][:third_pairs]
+    third = np.full(n, -1, np.int32)
+    for q, (a, b) in enumerate(pairs):
+        third[2 * q], third[2 * q + 1] = a, b
+    return dict(cur=cur, targets=targets, entries=entries, target_point=target_point, points=points, cur_point=cur_point,
+                cand=np.asarray(cand, np.int32), conn=conn, third_point=third, boundary_rows=np.asarray(boundary_rows, np.int64))
+
+
+def fuse_scene_arrays(sc):
+    """The parts of a make_fuse_scene dict that api.fuse_neighbours reads, as flat named arrays (for np.savez)"""
+    out = dict(cur_point=sc["cur_point"], cand=sc["cand"], n_targets=np.int64(len(sc["targets"])))
+    for k, v in sc["points"].items():
+        out["points_" + k] = np.asarray(v)
+    for i, kf in enumerate([sc["cur"]] + list(sc["targets"])):
+        for k in ("desc", "kp_xy", "octave", "angle", "bounds", "cols", "rows", "intr", "Tcw", "Ow", "scale_factors", "inv_level_sigma2",
+                  "log_scale_factor"):
+            out["kf%d_%s" % (i, k)] = np.asarray(kf[k])
+    return out
+
+
+def fuse_scene_from_arrays(z):
+    """inverse of fuse_scene_arrays"""
+    kfs = []
+    for i in range(1 + int(z["n_targets"])):
+        kf = {k: z["kf%d_%s" % (i, k)] for k in ("desc", "kp_xy", "octave", "angle", "intr", "Tcw", "Ow", "scale_factors", "inv_level_sigma2")}
+        kf["bounds"] = tuple(float(b) for b in z["kf%d_bounds" % i])
+        kf["cols"], kf["rows"] = int(z["kf%d_cols" % i]), int(z["kf%d_rows" % i])
+        kf["log_scale_factor"] = np.float32(z["kf%d_log_scale_factor" % i])
+        kfs.append(kf)
+    points = {k[len("points_"):]: z[k] for k in z.files if k.startswith("points_")}
+    return dict(cur=kfs[0], targets=kfs[1:], points=points, cur_point=z["cur_point"], cand=z["cand"])

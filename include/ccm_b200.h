@@ -798,6 +798,61 @@ int ccm_new_map_points(const ccm_newpts_view* cur, const ccm_newpts_neighbour* n
 int ccm_new_map_points_host(const ccm_newpts_view* cur, const ccm_newpts_neighbour* nb, int32_t n_nb, ccm_new_point* out, int32_t capacity,
                             int32_t* n_out, int32_t* best2, uint8_t* verdict);
 
+/* ---- neighbour fusion ---------------------------------------------------------------------------------------------------
+ * The searches of LocalMapping::SearchInNeighbors (cslam/src/Mapping.cpp:471-547) in one call.  The member runs
+ * ORBmatcher::Fuse(pKFi, vpMapPointMatches) (cslam/src/ORBmatcher.cpp:854-993, th = 3) for every fuse target in list order (forward),
+ * then Fuse(mpCurrentKeyFrame, vpFuseCandidates) once (backward).  The target list (first neighbours, their second neighbours, the
+ * mFuseTargetForKF marks), the candidate list (mFuseCandidateForKF) and all map surgery stay with the caller.
+ *
+ * Why one pass is enough: every backward candidate is a target's point when the member starts, and the search part of Fuse reads
+ * no map state that the surgery changes except isBad(), IsInKeyFrame() and, through MapPoint::Replace, the surviving point's
+ * descriptor.  So every pair is searched here over the state at the start of the member; the caller walks the reference's order,
+ * checks isBad() / IsInKeyFrame() live, and searches again on the host (ccm_fuse_select) only a pair whose point's descriptor no
+ * longer equals the bytes passed in.
+ *
+ * Each (keyframe, point) pair runs Fuse's prelude (projection, IsInImage, the distance-invariance range, the 60-degree cone,
+ * PredictScale; ccm_slam_b200/csrc/fuse_neighbours_math.cuh) and its window search: levels [L-1, L], the chi-square gate on
+ * mvInvLevelSigma2, the first minimum of the Hamming distance, kept when <= TH_LOW.  PredictScale's log(float) is glibc's logf, which
+ * the device does not reproduce; a pair whose level depends on the last bit of that logarithm is settled on the host with the host's
+ * logf before the call returns (DESIGN.md §5).  *n_settled (may be NULL) counts those pairs.
+ *
+ * In:  cur              the current keyframe; targets[0..n_targets) the DISTINCT fuse targets (a target listed twice is passed once);
+ *      pts              the point table; a point with skip set (mbDoNotReplace, or isBad() on entry) is never searched;
+ *      cur_point[i]     the point row of the current keyframe's slot i (vpMapPointMatches[i]), -1 for an empty slot, cur->grid.n entries;
+ *      cand[0..n_cand)  the point rows of vpFuseCandidates, in order.
+ * Out: fwd_best[t * cur->grid.n + i]   keypoint of target t that slot i's point fuses with, or -1;
+ *      bwd_best[c]                     keypoint of the current keyframe that candidate c fuses with, or -1.
+ * A row out of range, a null array or a grid with more keypoints than the 20-bit visiting position of the window key holds fails
+ * with CCM_ERR_INVALID and a message naming the target, slot or candidate; nothing is written.
+ * ccm_fuse_neighbours: one upload, one launch whatever the number of targets, one download; no atomics, identical bytes every call.
+ * ccm_fuse_neighbours_host: the same contract without a device; the two agree bit for bit. */
+typedef struct ccm_fuse_kf {          /* one keyframe as Fuse reads it */
+  ccm_feature_grid grid;              /* mvKeysUn, mDescriptors and the lookup grid; min_x .. max_y are also IsInImage's bounds */
+  float Tcw[12];                      /* [Rcw | tcw], 3x4 row-major f32 */
+  float Ow[3];                        /* GetCameraCenter() */
+  float fx, fy, cx, cy;
+  const float* scale_factors;         /* mvScaleFactors, nlevels */
+  const float* inv_level_sigma2;      /* mvInvLevelSigma2, nlevels */
+  int32_t nlevels;                    /* mnScaleLevels */
+  float log_scale_factor;             /* mfLogScaleFactor */
+} ccm_fuse_kf;
+typedef struct ccm_fuse_points {      /* the map points the call may search, one row each */
+  int32_t n;
+  const float* pos;                   /* n*3 GetWorldPos() */
+  const float* normal;                /* n*3 GetNormal() */
+  const float* max_distance;          /* n   mfMaxDistance (the member's gate uses 1.2f times it, PredictScale the value itself) */
+  const float* min_distance;          /* n   mfMinDistance */
+  const uint8_t* desc;                /* n*32 GetDescriptor() */
+  const uint8_t* skip;                /* n   mbDoNotReplace || isBad() */
+} ccm_fuse_points;
+
+int ccm_fuse_neighbours(const ccm_fuse_kf* cur, const ccm_fuse_kf* targets, int32_t n_targets, const ccm_fuse_points* pts,
+                        const int32_t* cur_point, const int32_t* cand, int32_t n_cand, int32_t* fwd_best, int32_t* bwd_best,
+                        int32_t* n_settled);
+int ccm_fuse_neighbours_host(const ccm_fuse_kf* cur, const ccm_fuse_kf* targets, int32_t n_targets, const ccm_fuse_points* pts,
+                             const int32_t* cur_point, const int32_t* cand, int32_t n_cand, int32_t* fwd_best, int32_t* bwd_best,
+                             int32_t* n_settled);
+
 #ifdef __cplusplus
 }
 #endif
