@@ -603,6 +603,44 @@ def covisibility(sc, th=15, host=False, capacity=None, batch=None):
         out[k] = out[k][:T]
     return out
 
+SIM3_CORRECTION_IN = (("kf_centre", np.float32), ("kf_bad", np.uint8), ("entry_kf", np.int32), ("entry_Siw_new", np.float64),
+                      ("entry_Siw_old", np.float64), ("slot_ptr", np.int64), ("slot_mp", np.int32), ("mp_pos", np.float32),
+                      ("mp_skip", np.uint8), ("obs_ptr", np.int64), ("obs_kf", np.int32), ("mp_ref", np.int32), ("mp_scale_ref", np.float32),
+                      ("mp_scale_last", np.float32))
+
+
+def sim3_correction_out(n_e, n_mp):
+    """zeroed outputs of ccm_sim3_correction for n_e entries and n_mp points"""
+    return dict(entry_Tcw=np.zeros((n_e, 4, 4), np.float32), entry_centre=np.zeros((n_e, 3), np.float32), mp_entry=np.zeros(n_mp, np.int32),
+                mp_pos=np.zeros((n_mp, 3), np.float32), normal=np.zeros((n_mp, 3), np.float32), max_dist=np.zeros(n_mp, np.float32),
+                min_dist=np.zeros(n_mp, np.float32), status=np.zeros(n_mp, np.uint8))
+
+
+def sim3_correction_args(sc, out):
+    """(argument tuple of ccm_sim3_correction, arrays it points into) for a scene as synth.make_sim3_correction builds it"""
+    a = {k: np.ascontiguousarray(sc[k], t) for k, t in SIM3_CORRECTION_IN}
+    K, E, P = len(a["kf_bad"]), len(a["entry_kf"]), len(a["mp_skip"])
+    argv = (K, _p(a["kf_centre"]), _p(a["kf_bad"]), E, _p(a["entry_kf"]), _p(a["entry_Siw_new"]), _p(a["entry_Siw_old"]), _p(a["slot_ptr"]),
+            _p(a["slot_mp"]), P, _p(a["mp_pos"]), _p(a["mp_skip"]), _p(a["obs_ptr"]), _p(a["obs_kf"]), _p(a["mp_ref"]), _p(a["mp_scale_ref"]),
+            _p(a["mp_scale_last"]), _p(out["entry_Tcw"]), _p(out["entry_centre"]), _p(out["mp_entry"]), _p(out["mp_pos"]), _p(out["normal"]),
+            _p(out["max_dist"]), _p(out["min_dist"]), _p(out["status"]))
+    return argv, a
+
+
+def sim3_correction(sc, host=False, out=None):
+    """The Sim3 correction pass of LoopFinder::CorrectLoop / MapMerger::MergeMaps (cslam/src/LoopFinder.cpp:568-613,
+    cslam/src/MapMerger.cpp:349-395), see include/ccm_b200.h.  sc: dict(kf_centre (K,3) f32, kf_bad (K,) u8, entry_kf (E,) i32,
+    entry_Siw_new / entry_Siw_old (E,8) f64, slot_ptr (E+1,) i64, slot_mp i32, mp_pos (P,3) f32, mp_skip (P,) u8, obs_ptr (P+1,) i64,
+    obs_kf i32, mp_ref (P,) i32, mp_scale_ref / mp_scale_last (P,) f32), as synth.make_sim3_correction builds it.  Returns dict(entry_Tcw
+    (E,4,4) f32, entry_centre (E,3), mp_entry (P,) i32, mp_pos (P,3), normal (P,3), max_dist, min_dist, status).  host=False:
+    ccm_sim3_correction on the GPU; host=True: ccm_sim3_correction_host.  out: preallocated outputs (sim3_correction_out)."""
+    out = sim3_correction_out(len(sc["entry_kf"]), len(sc["mp_skip"])) if out is None else out
+    argv, _keep = sim3_correction_args(sc, out)
+    fn = lib().ccm_sim3_correction_host if host else lib().ccm_sim3_correction
+    _chk(fn(*argv))
+    return out
+
+
 class NewPtsViewC(C.Structure):
     _fields_ = [("v", TriViewC), ("Tcw", C.c_float * 12), ("Ow", C.c_float * 3), ("level_sigma2", C.c_void_p),
                 ("scale_factors", C.c_void_p), ("nlevels", C.c_int32), ("scale_factor", C.c_float)]

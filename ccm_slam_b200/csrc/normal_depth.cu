@@ -32,7 +32,7 @@ __global__ void __launch_bounds__(256) k_normal_depth(int n, int n_kf, const flo
     uint8_t st = 0;
     if (ok) {
       const float X[3] = {pos[3 * (size_t)i], pos[3 * (size_t)i + 1], pos[3 * (size_t)i + 2]};
-      st = nd::update_point(X, obs_kf, b, e, centre, kf_bad, r, scale_ref[i], scale_last[i], nv, &dmax, &dmin);
+      st = nd::update_point(X, obs_kf, b, e, nd::TableCentres{centre}, kf_bad, r, scale_ref[i], scale_last[i], nv, &dmax, &dmin);
     } else {
       atomicExch(bad_index, 1);
     }
@@ -71,7 +71,7 @@ extern "C" int ccm_normal_depth_host(int32_t n_kf, const float* kf_centre, const
     }
     for (int32_t i = 0; i < n_mp; i++) {
       float* nv = normal + 3 * (size_t)i;
-      const uint8_t st = nd::update_point(mp_pos + 3 * (size_t)i, obs_kf, obs_ptr[i], obs_ptr[i + 1], kf_centre, kf_bad, mp_ref[i],
+      const uint8_t st = nd::update_point(mp_pos + 3 * (size_t)i, obs_kf, obs_ptr[i], obs_ptr[i + 1], nd::TableCentres{kf_centre}, kf_bad, mp_ref[i],
                                           mp_scale_ref[i], mp_scale_last[i], nv, max_dist + i, min_dist + i);
       if (!st) { nv[0] = nv[1] = nv[2] = 0.f; max_dist[i] = min_dist[i] = 0.f; }
       status[i] = st;

@@ -103,11 +103,20 @@ CCM_ND_HD double norm3(const float d[3]) {
 #endif
 }
 
-// One point.  X its position; obs_kf[b..e) its observers' keyframe rows in mObservations order; centre [K][3] / bad [K] the keyframe table;
-// ref the row of mpRefKF; scale_ref = mvScaleFactors[octave of the reference observation], scale_last = mvScaleFactors[nLevels-1].
+// The centre lookup of update_point when every keyframe reads its row of one [K][3] table (ccm_normal_depth).  The Sim3 correction
+// (sim3_correction_math.cuh) passes its own lookup instead: there a keyframe's centre depends on the point being corrected.
+struct TableCentres {
+  const float* centre;
+  CCM_ND_HD void operator()(int32_t k, float O[3]) const { centre_of(centre, k, O); }
+};
+
+// One point.  X its position; obs_kf[b..e) its observers' keyframe rows in mObservations order; centre_at(k, O) writes GetCameraCenter()
+// of keyframe row k as this point sees it; bad [K] the keyframe flags; ref the row of mpRefKF; scale_ref = mvScaleFactors[octave of the
+// reference observation], scale_last = mvScaleFactors[nLevels-1].
 // Returns 1 and writes the three members, or 0 (no observers or no reference keyframe: the reference returns before writing).
-CCM_ND_HD uint8_t update_point(const float X[3], const int32_t* obs_kf, int64_t b, int64_t e, const float* centre, const uint8_t* bad, int32_t ref,
-                               float scale_ref, float scale_last, float normal[3], float* max_dist, float* min_dist) {
+template <typename Centres>
+CCM_ND_HD uint8_t update_point(const float X[3], const int32_t* obs_kf, int64_t b, int64_t e, const Centres& centre_at, const uint8_t* bad,
+                               int32_t ref, float scale_ref, float scale_last, float normal[3], float* max_dist, float* min_dist) {
   if (b >= e || ref < 0) return 0;
   float nv[3] = {0.f, 0.f, 0.f};
   int n = 0;
@@ -115,7 +124,7 @@ CCM_ND_HD uint8_t update_point(const float X[3], const int32_t* obs_kf, int64_t 
     const int32_t k = obs_kf[j];
     if (bad[k]) continue;
     float O[3];
-    centre_of(centre, k, O);
+    centre_at(k, O);
     const float d[3] = {fsub(X[0], O[0]), fsub(X[1], O[1]), fsub(X[2], O[2])};
     const float a = to_f32(drcp(norm3(d)));
     nv[0] = ffma(d[0], a, nv[0]);
@@ -124,7 +133,7 @@ CCM_ND_HD uint8_t update_point(const float X[3], const int32_t* obs_kf, int64_t 
     n++;
   }
   float O[3];
-  centre_of(centre, ref, O);
+  centre_at(ref, O);
   const float pc[3] = {fsub(X[0], O[0]), fsub(X[1], O[1]), fsub(X[2], O[2])};
   const float dist = to_f32(norm3(pc));
   *max_dist = fmul(dist, scale_ref);

@@ -646,3 +646,149 @@ def make_covisibility(p: BAProblem | None = None, seed=0, K=60, P=2000, max_deg=
     batch = np.arange(K) if batch_frac >= 1 else np.sort(rng.choice(K, max(1, int(K * batch_frac)), replace=False))
     return covis_pack(K, kf, mp, P, rng, kf_id=kf_id, null_frac=null_frac, dup_frac=dup_frac, bad_mp_frac=bad_mp_frac,
                       bad_kf_frac=bad_kf_frac, batch=batch)
+
+
+def _eigen_quat(R):
+    """Eigen's Quaterniond(Matrix3d) (vectorised, f64): the branches of ba_math.cuh's R_to_quat, no normalisation, as
+    g2o::Sim3(R, t, s) keeps it.  R (n,3,3) -> (n,4) qx qy qz qw"""
+    R = np.asarray(R, np.float64).reshape(-1, 3, 3)
+    q = np.zeros((len(R), 4))
+    for i in range(len(R)):
+        m = R[i]
+        t = m[0, 0] + m[1, 1] + m[2, 2]
+        if t > 0:
+            t = np.sqrt(t + 1.0); w = 0.5 * t; t = 0.5 / t
+            q[i] = [(m[2, 1] - m[1, 2]) * t, (m[0, 2] - m[2, 0]) * t, (m[1, 0] - m[0, 1]) * t, w]
+        else:
+            a = 0 if (m[0, 0] >= m[1, 1] and m[0, 0] >= m[2, 2]) else (1 if m[1, 1] >= m[2, 2] else 2)
+            b, c = (a + 1) % 3, (a + 2) % 3
+            t = np.sqrt(m[a, a] - m[b, b] - m[c, c] + 1.0)
+            v = np.zeros(3); v[a] = 0.5 * t; t = 0.5 / t
+            w = (m[c, b] - m[b, c]) * t; v[b] = (m[b, a] + m[a, b]) * t; v[c] = (m[c, a] + m[a, c]) * t
+            q[i] = [v[0], v[1], v[2], w]
+    return q
+
+
+def _f32_gemm4(A, B):
+    """A @ B for f32 4x4 stacks, each element summed left to right in f32 (cv::gemm's small-matrix path)"""
+    A = np.asarray(A, np.float32); B = np.asarray(B, np.float32)
+    C = A[..., :, 0:1] * B[..., 0:1, :]
+    for k in range(1, 4):
+        C = (C + A[..., :, k:k + 1] * B[..., k:k + 1, :]).astype(np.float32)
+    return C
+
+
+def _f32_pose_inverse(T):
+    """KeyFrame::SetPose's Twc from f32 Tcw stacks: [R^T | -(R^T t)], the product summed left to right in f32"""
+    T = np.asarray(T, np.float32)
+    R, t = T[..., :3, :3], T[..., :3, 3]
+    ow = R[..., 0, :] * t[..., 0:1]
+    ow = (ow + R[..., 1, :] * t[..., 1:2]).astype(np.float32)
+    ow = (ow + R[..., 2, :] * t[..., 2:3]).astype(np.float32)
+    W = np.zeros(T.shape, np.float32)
+    W[..., :3, :3] = np.swapaxes(R, -1, -2); W[..., :3, 3] = -ow; W[..., 3, 3] = 1
+    return W
+
+
+def make_sim3_correction(p: BAProblem | None = None, kind="loop", seed=0, K=60, P=2000, max_deg=8, window=12, n_loop=30, null_frac=0.05,
+                         dup_frac=0.02, bad_mp_frac=0.03, tagged_frac=0.03, bad_kf_frac=0.05, all_bad_frac=0.0, off_ref_frac=0.05,
+                         no_ref_frac=0.0, empty_frac=0.0, null_entry_frac=0.0, unlisted_frac=0.0, scale=1.07):
+    """Inputs of ccm_sim3_correction (the Sim3 pass of LoopFinder::CorrectLoop / MapMerger::MergeMaps, include/ccm_b200.h) over the map
+    of a BA problem `p` (None: K keyframes and P points, 1..max_deg observers each drawn from a window of `window` consecutive rows).
+    f32 poses and centres as SetPose leaves them; mvpMapPoints and observer lists from covis_pack (null slots, a point at two slots, bad
+    points and keyframes); address ranks a random permutation, so the entries' map order differs from their row order.
+    kind="merge": every keyframe is an entry (CorrectedSim3All); kind="loop": a current keyframe and its n_loop most covisible
+    keyframes (CorrectedSim3), so observers and reference keyframes fall before, after, on and outside the entries.
+    Corrected Sim3s as the sites build them: the current keyframe's Scw = (drift correction with scale `scale`) * Sim3(Tcw, 1);
+    for the others Sic = Sim3(R, t, 1) of the f32 product Tiw*Twc and CorrectedSiw = Sic * Scw; NonCorrectedSim3 = Sim3(Riw, tiw, 1).
+    Knobs: tagged_frac (points already tagged with the current mId, passed as skipped), all_bad_frac (points whose observers are all bad),
+    off_ref_frac (mpRefKF any keyframe), no_ref_frac (no mpRefKF), empty_frac (entries with no slots), null_entry_frac (entries whose
+    slots are all null), unlisted_frac (slots turned null while the point keeps the observation: an entry that observes a point
+    without listing it, so that observers fall before the claiming entry).  Extra keys: kf_Tcw (K,4,4) f32, kf_rank, mp_bad, mp_tagged, cur (row of the current keyframe)."""
+    rng = np.random.default_rng(seed)
+    if p is None:
+        Rcw, tcw, C, zc = _helix_cameras(K, rng, radius=6.0, dtheta=0.05, dz=0.01)
+        Tcw = np.tile(np.eye(4), (K, 1, 1)); Tcw[:, :3, :3] = Rcw; Tcw[:, :3, 3] = tcw
+        deg = rng.integers(1, max_deg + 1, P)
+        mp = np.repeat(np.arange(P, dtype=np.int64), deg)
+        start = rng.integers(0, max(K - window, 1), P)
+        kf = np.repeat(start, deg) + rng.integers(0, min(window, K), len(mp))
+        base = np.clip(start + min(window, K) // 2, 0, K - 1)
+        pos = C[base] + zc[base] * rng.uniform(2.0, 8.0, (P, 1)) + rng.normal(0, 1.0, (P, 3))
+    else:
+        K, P = p.K, p.P
+        q = p.poses[:, :4]; x, y, z, w = q[:, 0], q[:, 1], q[:, 2], q[:, 3]
+        R = np.stack([1 - 2 * (y * y + z * z), 2 * (x * y - z * w), 2 * (x * z + y * w),
+                      2 * (x * y + z * w), 1 - 2 * (x * x + z * z), 2 * (y * z - x * w),
+                      2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)], 1).reshape(K, 3, 3)
+        Tcw = np.tile(np.eye(4), (K, 1, 1)); Tcw[:, :3, :3] = R; Tcw[:, :3, 3] = p.poses[:, 4:7]
+        kf, mp = p.obs_kf.astype(np.int64), p.obs_mp.astype(np.int64)
+        pos = p.points
+    Tcw = Tcw.astype(np.float32)
+    cen = _f32_pose_inverse(Tcw)[:, :3, 3].copy()
+    pk = covis_pack(K, kf, mp, P, rng, null_frac=null_frac, dup_frac=dup_frac, bad_mp_frac=bad_mp_frac, bad_kf_frac=bad_kf_frac)
+    rank = pk["kf_rank"].astype(np.int64)
+    obs_ptr, obs_kf = pk["obs_ptr"], pk["obs_kf"].copy()
+    deg = np.diff(obs_ptr)
+    kf_bad = pk["kf_bad"]
+    cur = int(rng.integers(0, K))
+    if kind == "merge":
+        rows = np.arange(K)
+    elif kind == "loop":
+        # the current keyframe and its most covisible keyframes (shared points)
+        mine = pk["mvp"][pk["mvp_ptr"][cur]:pk["mvp_ptr"][cur + 1]]
+        mine = np.unique(mine[mine >= 0])
+        sel = np.concatenate([obs_kf[obs_ptr[i]:obs_ptr[i + 1]] for i in mine]) if len(mine) else np.zeros(0, np.int64)
+        cnt = np.bincount(sel, minlength=K); cnt[cur] = 0
+        nb = np.argsort(-cnt, kind="stable")[:n_loop]
+        rows = np.concatenate([[cur], nb[cnt[nb] > 0]])
+    else:
+        raise ValueError(kind)
+    entry_kf = rows[np.argsort(rank[rows], kind="stable")].astype(np.int32)     # std::map<kfptr> order
+    E = len(entry_kf)
+    # corrected Sim3s as the sites build them
+    corr_q = _rotvec_to_quat(rng.normal(0, 0.05, 3)); corr_q = corr_q / np.linalg.norm(corr_q)
+    S_corr = np.concatenate([corr_q, rng.normal(0, 0.3, 3), [scale]])
+    Tc = Tcw[cur].astype(np.float64)
+    S_cur = np.concatenate([_eigen_quat(Tc[:3, :3])[0], Tc[:3, 3], [1.0]])
+    Scw = _sim3_mul(S_corr, S_cur)
+    Twc = _f32_pose_inverse(Tcw[cur])
+    Tic = _f32_gemm4(Tcw[entry_kf], Twc)
+    Sic = np.concatenate([_eigen_quat(Tic[:, :3, :3].astype(np.float64)), Tic[:, :3, 3].astype(np.float64), np.ones((E, 1))], 1)
+    Siw_new = np.array([Scw if k == cur else _sim3_mul(Sic[e], Scw) for e, k in enumerate(entry_kf)]).reshape(E, 8)
+    Siw_old = np.concatenate([_eigen_quat(Tcw[entry_kf, :3, :3].astype(np.float64)), Tcw[entry_kf, :3, 3].astype(np.float64),
+                              np.ones((E, 1))], 1)
+    # slots: each entry's mvpMapPoints
+    mptr, mvp = pk["mvp_ptr"], pk["mvp"]
+    lists = [mvp[mptr[k]:mptr[k + 1]].copy() for k in entry_kf]
+    for e in range(E):
+        lists[e][rng.random(len(lists[e])) < unlisted_frac] = -1
+        u = rng.random()
+        if u < empty_frac:
+            lists[e] = lists[e][:0]
+        elif u < empty_frac + null_entry_frac:
+            lists[e][:] = -1
+    slot_ptr = np.zeros(E + 1, np.int64); slot_ptr[1:] = np.cumsum([len(s) for s in lists])
+    slot_mp = np.concatenate(lists).astype(np.int32) if E else np.zeros(0, np.int32)
+    # points
+    mp_bad = pk["mp_bad"].astype(bool)
+    tagged = rng.random(P) < tagged_frac
+    bad_rows = np.flatnonzero(kf_bad)
+    if len(bad_rows):
+        for i in np.flatnonzero((rng.random(P) < all_bad_frac) & (deg > 0) & (deg <= len(bad_rows))):
+            pick = rng.choice(bad_rows, deg[i], replace=False)
+            obs_kf[obs_ptr[i]:obs_ptr[i + 1]] = pick[np.argsort(rank[pick])]
+    sf = scale_factors()
+    ref = np.full(P, -1, np.int32)
+    has = deg > 0
+    pick = obs_ptr[:-1] + (rng.random(P) * np.maximum(deg, 1)).astype(np.int64)
+    ref[has] = obs_kf[pick[has]]
+    off = has & (rng.random(P) < off_ref_frac)
+    ref[off] = rng.integers(0, K, int(off.sum()))
+    ref[rng.random(P) < no_ref_frac] = -1
+    sref = sf[rng.choice(8, P, p=OCTAVE_QUOTAS / OCTAVE_QUOTAS.sum())].astype(np.float32)
+    return dict(kf_centre=cen.astype(np.float32), kf_bad=kf_bad.astype(np.uint8), entry_kf=entry_kf, entry_Siw_new=Siw_new,
+                entry_Siw_old=Siw_old, slot_ptr=slot_ptr, slot_mp=slot_mp, mp_pos=np.asarray(pos, np.float32),
+                mp_skip=(mp_bad | tagged).astype(np.uint8), obs_ptr=obs_ptr, obs_kf=obs_kf.astype(np.int32), mp_ref=ref,
+                mp_scale_ref=sref, mp_scale_last=np.full(P, sf[-1], np.float32), kf_Tcw=Tcw, kf_rank=pk["kf_rank"], mp_bad=mp_bad,
+                mp_tagged=tagged, cur=cur)

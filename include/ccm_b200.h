@@ -853,6 +853,38 @@ int ccm_fuse_neighbours_host(const ccm_fuse_kf* cur, const ccm_fuse_kf* targets,
                              const int32_t* cur_point, const int32_t* cand, int32_t n_cand, int32_t* fwd_best, int32_t* bwd_best,
                              int32_t* n_settled);
 
+/* ---- Sim3 correction of a loop closure or a map merge ---------------------------------------------------------------------
+ * The pass over CorrectedSim3 of LoopFinder::CorrectLoop (cslam/src/LoopFinder.cpp:568-613) and over CorrectedSim3All of
+ * MapMerger::MergeMaps (cslam/src/MapMerger.cpp:349-395), bit for bit (f64 Sim3 arithmetic in Eigen's order, f32 where the reference
+ * stores; see ccm_slam_b200/csrc/sim3_correction_math.cuh).  Entry e is the e-th element of the std::map in its iteration order.
+ *   kf_centre [n_kf][3]   GetCameraCenter() of each keyframe row before the pass;  kf_bad [n_kf]: isBad()
+ *   entry_kf [n_e]        the keyframe row of each entry (each row at most once)
+ *   entry_Siw_new [n_e][8], entry_Siw_old [n_e][8]   the entry's corrected Sim3 and NonCorrectedSim3[pKFi], qx qy qz qw tx ty tz s
+ *   slot_ptr [n_e+1], slot_mp [slot_ptr[n_e]]        entry e's GetMapPointMatches() in index order as point rows, -1 = null
+ *   mp_pos [n_mp][3]      GetWorldPos();  mp_skip [n_mp]: isBad(), or mCorrectedByKF_LC / _MM already equal to the current mId
+ *   obs_ptr, obs_kf, mp_ref, mp_scale_ref, mp_scale_last   the observers, mpRefKF and scale factors exactly as ccm_normal_depth takes them
+ * Out, per entry: entry_Tcw [n_e][16] (row-major f32, the pose SetPose receives), entry_centre [n_e][3] (the Ow it leaves).
+ * Out, per point: mp_entry [n_mp]: the entry that moves the point (the first in map order that lists it, when it is not skipped), -1
+ * none; mp_pos_out [n_mp][3]: the corrected position (mp_pos for a point no entry moves); normal, max_dist, min_dist, status: what
+ * UpdateNormalAndDepth leaves right after the move, with ccm_normal_depth's semantics (0 everywhere and status 0 for a point no entry
+ * moves).  The normal reads the corrected centre of each keyframe that is an entry BEFORE mp_entry and the pre-loop centre of every
+ * other keyframe, mp_entry's own included: the reference's SetPose for an entry follows its points.
+ * A row out of range, a keyframe listed as two entries or a null array fails with CCM_ERR_INVALID and a message naming the entry, slot
+ * or point; nothing is written then.
+ * ccm_sim3_correction runs on the GPU (host buffers in and out, its own stream, three launches); ccm_sim3_correction_host is the same
+ * contract on the host, usable without a device. */
+int ccm_sim3_correction(int32_t n_kf, const float* kf_centre, const uint8_t* kf_bad, int32_t n_e, const int32_t* entry_kf,
+                        const double* entry_Siw_new, const double* entry_Siw_old, const int64_t* slot_ptr, const int32_t* slot_mp, int32_t n_mp,
+                        const float* mp_pos, const uint8_t* mp_skip, const int64_t* obs_ptr, const int32_t* obs_kf, const int32_t* mp_ref,
+                        const float* mp_scale_ref, const float* mp_scale_last, float* entry_Tcw, float* entry_centre, int32_t* mp_entry,
+                        float* mp_pos_out, float* normal, float* max_dist, float* min_dist, uint8_t* status);
+int ccm_sim3_correction_host(int32_t n_kf, const float* kf_centre, const uint8_t* kf_bad, int32_t n_e, const int32_t* entry_kf,
+                             const double* entry_Siw_new, const double* entry_Siw_old, const int64_t* slot_ptr, const int32_t* slot_mp,
+                             int32_t n_mp, const float* mp_pos, const uint8_t* mp_skip, const int64_t* obs_ptr, const int32_t* obs_kf,
+                             const int32_t* mp_ref, const float* mp_scale_ref, const float* mp_scale_last, float* entry_Tcw,
+                             float* entry_centre, int32_t* mp_entry, float* mp_pos_out, float* normal, float* max_dist, float* min_dist,
+                             uint8_t* status);
+
 #ifdef __cplusplus
 }
 #endif

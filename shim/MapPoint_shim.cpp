@@ -6,7 +6,9 @@
 //     points (observers in mObservations order, each keyframe's centre and isBad() read once), makes one ccm_normal_depth call on the
 //     GPU and parks the results per thread, with a snapshot of what they were computed from: position, observation count, pRefKF.
 //     The member then writes the parked values when the snapshot still matches;
-//   * single point: every other caller (tracking, mapping, the MapMerger / LoopFinder correction loops, the communicator) and any
+//   * parked by another batch: shim/Sim3Correction_shim.cpp computes the normals of the points a loop or merge correction moves in its
+//     own device call and parks them through ccm_b200_park_normals, under the same snapshot rule;
+//   * single point: every other caller (tracking, mapping, the communicator) and any
 //     point whose snapshot went stale computes on the host through ccm_normal_depth_host, the same arithmetic.
 // In this repository it is compiled against the stand-in MapPoint / KeyFrame of oracle/ref_stub_mp and run next to a literal
 // restatement of the reference body by tests/test_normal_depth.py.
@@ -82,6 +84,19 @@ void check(int rc, const char* fn) {
 // member calls by outcome, process-wide: a parked value written / a parked value found stale / computed on the host
 std::atomic<unsigned long long> g_hits(0), g_stale(0), g_host(0);
 
+// parks the values of point i (status[i] != 0) with the snapshot snap[i] (observation count, pRefKF) and the position pos[i]
+void park(const std::vector<const MapPoint*>& who, const float* pos, std::vector<Parked>& snap, const float* normal, const float* dmax,
+          const float* dmin, const uint8_t* status) {
+  std::unordered_map<const MapPoint*, Parked>& t = parked();
+  for (size_t i = 0; i < who.size(); i++) {
+    if (!status[i]) continue;
+    Parked& p = snap[i];
+    for (int j = 0; j < 3; j++) { p.pos[j] = pos[3 * i + j]; p.normal[j] = normal[3 * i + j]; }
+    p.max_dist = dmax[i]; p.min_dist = dmin[i];
+    t[who[i]] = p;
+  }
+}
+
 }  // namespace
 
 void ccm_b200_prepare_normals(const std::vector<mpptr>& points, const float* new_pos) {
@@ -110,14 +125,28 @@ void ccm_b200_prepare_normals(const std::vector<mpptr>& points, const float* new
   check(ccm_normal_depth((int32_t)f.bad.size(), f.centre.data(), f.bad.data(), P, f.pos.data(), f.ptr.data(), f.obs.data(), f.ref.data(),
                          f.scale_ref.data(), f.scale_last.data(), normal.data(), dmax.data(), dmin.data(), status.data()),
         "ccm_normal_depth");
-  std::unordered_map<const MapPoint*, Parked>& t = parked();
-  for (int32_t i = 0; i < P; i++) {
-    if (!status[i]) continue;
-    Parked& p = snap[i];
-    for (int j = 0; j < 3; j++) p.normal[j] = normal[3 * (size_t)i + j];
-    p.max_dist = dmax[i]; p.min_dist = dmin[i];
-    t[who[i]] = p;
+  park(who, f.pos.data(), snap, normal.data(), dmax.data(), dmin.data(), status.data());
+}
+
+void ccm_b200_park_normals(const std::vector<mpptr>& points, const float* pos, const float* normal, const float* max_dist,
+                           const float* min_dist, const uint8_t* status) {
+  std::vector<const MapPoint*> who;
+  std::vector<Parked> snap;
+  std::vector<float> p_pos, p_normal, p_max, p_min;
+  std::vector<uint8_t> p_status;
+  for (size_t i = 0; i < points.size(); i++) {
+    const mpptr& pMP = points[i];
+    if (!pMP || !status[i]) continue;
+    Parked p;
+    p.n_obs = pMP->GetObservations().size();
+    p.ref = pMP->GetReferenceKeyFrame().get();
+    who.push_back(pMP.get());
+    snap.push_back(p);
+    p_pos.insert(p_pos.end(), pos + 3 * i, pos + 3 * i + 3);
+    p_normal.insert(p_normal.end(), normal + 3 * i, normal + 3 * i + 3);
+    p_max.push_back(max_dist[i]); p_min.push_back(min_dist[i]); p_status.push_back(1);
   }
+  park(who, p_pos.data(), snap, p_normal.data(), p_max.data(), p_min.data(), p_status.data());
 }
 
 void ccm_b200_clear_normals() { parked().clear(); }

@@ -1,6 +1,8 @@
 // MapPoint_shim.h — the batch entry of shim/MapPoint_shim.cpp, for the write-back loops of shim/Optimizer_shim.cpp.
 #ifndef CCM_MAPPOINT_SHIM_H
 #define CCM_MAPPOINT_SHIM_H
+#include <stdint.h>
+
 #include <vector>
 
 #include <boost/shared_ptr.hpp>
@@ -14,6 +16,11 @@ class MapPoint;
 // points before that call (nullptr: their current positions).  A parked value is used only while the point's position, observation
 // count and reference keyframe still match; the member computes on the host otherwise.
 void ccm_b200_prepare_normals(const std::vector<boost::shared_ptr<MapPoint> >& points, const float* new_pos);
+// Parks values computed elsewhere for the MapPoint::UpdateNormalAndDepth() calls that follow, under the same snapshot rule: point i
+// (status[i] != 0) gets normal [i][3], max_dist[i], min_dist[i], used while its position is pos[i][3] and its observation count and
+// reference keyframe are what they are now.  ccm_b200_prepare_normals parks its own results through the same table.
+void ccm_b200_park_normals(const std::vector<boost::shared_ptr<MapPoint> >& points, const float* pos, const float* normal,
+                           const float* max_dist, const float* min_dist, const uint8_t* status);
 // Drops every value parked on this thread.
 void ccm_b200_clear_normals();
 // Counts of MapPoint::UpdateNormalAndDepth() calls since the process started, by how they ended: a parked value written, a parked
