@@ -395,9 +395,13 @@ __global__ void __launch_bounds__(1024) k_sum_partials(const double* __restrict_
 // entry -> row dependence costs one memory latency per batch instead of two.  On H100 the kernel is bound by the rows it keeps in
 // flight: the 2 * UNROLL rows of a batch are requested together, and UNROLL 16 at 66 registers runs a cfg5 launch in 9.6 ms against
 // 11.3 at UNROLL 8 (48 registers), 10.0 at 32 and 12.7 at 4 (H100 80GB HBM3, 700 W).  (dmma_884: pcg.cuh)
+// The explicit minimum of one CTA per SM in the launch bounds lets ptxas hold every row of a batch in its own registers (96, five
+// CTAs = 20 warps per SM) instead of squeezing the batch into 66 (seven CTAs): fewer warps, but each keeps all 32 rows of its batch in
+// flight, and a cfg5 launch takes 8.3-8.6 ms against 9.5.  Capping it at 64 registers for 32 warps per SM (128, 64, 32 or 256-thread
+// CTAs) gives 9.7-10.9 ms (H100 80GB HBM3, 700 W).
 
 constexpr int SCHUR_CTA = 128;   // threads per CTA of k_schur_mma: 4 upper blocks
-__global__ void __launch_bounds__(SCHUR_CTA) k_schur_mma(const uint2* __restrict__ prod, const unsigned* __restrict__ u_prod_ptr,
+__global__ void __launch_bounds__(SCHUR_CTA, 1) k_schur_mma(const uint2* __restrict__ prod, const unsigned* __restrict__ u_prod_ptr,
                                                          const int* __restrict__ u_row, const int* __restrict__ u_col, int nub,
                                                          const double* __restrict__ Z, const int* __restrict__ o_lm,
                                                          const double* __restrict__ gvec, double* __restrict__ U_val,
