@@ -743,26 +743,33 @@ def fuse_structs(sc, keep):
     the call.  A keyframe: a grid dict (desc, kp_xy, octave, angle, bounds, cols, rows) plus Tcw (3,4), Ow, intr (fx, fy, cx, cy),
     scale_factors, inv_level_sigma2, log_scale_factor.  sc: cur, targets (distinct keyframes), points dict(pos (P,3), normal (P,3),
     max_d, min_d, desc (P,32), skip), cur_point (n,) and cand rows."""
-    def kf(k):
-        a = dict(sf=np.ascontiguousarray(k["scale_factors"], np.float32), il=np.ascontiguousarray(k["inv_level_sigma2"], np.float32))
-        keep.append(a)
-        fx, fy, cx, cy = (float(x) for x in k["intr"])
-        return FuseKfC(grid_struct(k, keep), (C.c_float * 12)(*np.asarray(k["Tcw"], np.float32).reshape(12)),
-                       (C.c_float * 3)(*np.asarray(k["Ow"], np.float32).reshape(3)), fx, fy, cx, cy, _p(a["sf"]), _p(a["il"]),
-                       len(a["sf"]), float(k["log_scale_factor"]))
-    cur = kf(sc["cur"])
+    cur = fuse_kf_struct(sc["cur"], keep)
     T = len(sc["targets"])
     tg = (FuseKfC * max(T, 1))()
     for i, k in enumerate(sc["targets"]):
-        tg[i] = kf(k)
-    p = sc["points"]
+        tg[i] = fuse_kf_struct(k, keep)
+    a = dict(cp=np.ascontiguousarray(sc["cur_point"], np.int32), cand=np.ascontiguousarray(sc["cand"], np.int32))
+    keep += [a, tg]
+    return cur, tg, T, fuse_points_struct(sc["points"], keep), a["cp"], a["cand"]
+
+
+def fuse_kf_struct(k, keep, Tcw="Tcw", Ow="Ow"):
+    """ccm_fuse_kf of one keyframe dict (see fuse_structs); Tcw / Ow name the keys the camera is read from"""
+    a = dict(sf=np.ascontiguousarray(k["scale_factors"], np.float32), il=np.ascontiguousarray(k["inv_level_sigma2"], np.float32))
+    keep.append(a)
+    fx, fy, cx, cy = (float(x) for x in k["intr"])
+    return FuseKfC(grid_struct(k, keep), (C.c_float * 12)(*np.asarray(k[Tcw], np.float32).reshape(12)),
+                   (C.c_float * 3)(*np.asarray(k[Ow], np.float32).reshape(3)), fx, fy, cx, cy, _p(a["sf"]), _p(a["il"]),
+                   len(a["sf"]), float(k["log_scale_factor"]))
+
+
+def fuse_points_struct(p, keep, skip="skip"):
+    """ccm_fuse_points of dict(pos (P,3), normal (P,3), max_d, min_d, desc (P,32), skip); `skip` names the key of the skip flags"""
     a = dict(pos=np.ascontiguousarray(p["pos"], np.float32).reshape(-1, 3), nrm=np.ascontiguousarray(p["normal"], np.float32).reshape(-1, 3),
              mx=np.ascontiguousarray(p["max_d"], np.float32), mn=np.ascontiguousarray(p["min_d"], np.float32),
-             desc=np.ascontiguousarray(p["desc"], np.uint8).reshape(-1, 32), skip=np.ascontiguousarray(p["skip"], np.uint8),
-             cp=np.ascontiguousarray(sc["cur_point"], np.int32), cand=np.ascontiguousarray(sc["cand"], np.int32))
-    keep += [a, tg]
-    pts = FusePointsC(len(a["mx"]), _p(a["pos"]), _p(a["nrm"]), _p(a["mx"]), _p(a["mn"]), _p(a["desc"]), _p(a["skip"]))
-    return cur, tg, T, pts, a["cp"], a["cand"]
+             desc=np.ascontiguousarray(p["desc"], np.uint8).reshape(-1, 32), skip=np.ascontiguousarray(p[skip], np.uint8))
+    keep.append(a)
+    return FusePointsC(len(a["mx"]), _p(a["pos"]), _p(a["nrm"]), _p(a["mx"]), _p(a["mn"]), _p(a["desc"]), _p(a["skip"]))
 
 
 def fuse_neighbours(sc, host=False, fn=None):
@@ -779,6 +786,31 @@ def fuse_neighbours(sc, host=False, fn=None):
     fn = fn or (lib().ccm_fuse_neighbours_host if host else lib().ccm_fuse_neighbours)
     _chk(fn(C.byref(cur), tg, T, C.byref(pts), _p(cp), _p(cand), len(cand), _p(fwd), _p(bwd), C.byref(settled)))
     return fwd, bwd, settled.value
+
+
+def search_and_fuse_structs(sc, keep, Tcw="Tcw", Ow="Ow", skip="skip"):
+    """The C structs of ccm_search_and_fuse for a scene as synth_match.make_search_and_fuse_scene builds it -> (kfs, n_kf, pts).
+    sc: kfs (keyframe dicts as fuse_structs takes them, Tcw / Ow the split of the corrected Scw), points (the loop points, skip = isBad())."""
+    K = len(sc["kfs"])
+    kfs = (FuseKfC * max(K, 1))()
+    for i, k in enumerate(sc["kfs"]):
+        kfs[i] = fuse_kf_struct(k, keep, Tcw, Ow)
+    keep.append(kfs)
+    return kfs, K, fuse_points_struct(sc["points"], keep, skip)
+
+
+def search_and_fuse(sc, host=False, fn=None):
+    """The searches of LoopFinder / MapMerger::SearchAndFuse (cslam/src/LoopFinder.cpp:709-734, MapMerger.cpp:574-598) for every
+    corrected keyframe in one call, see include/ccm_b200.h.  Returns (best (K, P) i32: keypoint of keyframe k that loop point i lands on,
+    or -1; the number of pairs whose PredictScale level was settled with the host's logf).
+    host=False: ccm_search_and_fuse on the GPU; host=True: ccm_search_and_fuse_host."""
+    keep = []
+    kfs, K, pts = search_and_fuse_structs(sc, keep)
+    best = np.full((K, pts.n), -3, np.int32)
+    settled = C.c_int32(-1)
+    fn = fn or (lib().ccm_search_and_fuse_host if host else lib().ccm_search_and_fuse)
+    _chk(fn(kfs, K, C.byref(pts), _p(best), C.byref(settled)))
+    return best, settled.value
 
 
 class MapMirror:

@@ -1,11 +1,13 @@
 // fuse_neighbours_math.cuh — the per-pair prelude of ORBmatcher::Fuse(kfptr, const vector<mpptr>&, th) (cslam/src/ORBmatcher.cpp:877-922)
-// as LocalMapping::SearchInNeighbors runs it (th = 3), shared by the kernel (fuse_neighbours.cu, nvcc) and the host entry point
-// ccm_fuse_neighbours_host (g++ -ffp-contract=off).  Every product and sum is one explicit rounding, so the device contracts nothing the
+// as LocalMapping::SearchInNeighbors runs it (th = 3), and of Fuse(kfptr, Scw, vpPoints, th, vpReplacePoint) (:1010-1069) as
+// SearchAndFuse runs it (th = 4, the camera from the caller's split of Scw).  Shared by the kernels (fuse_neighbours.cu,
+// search_and_fuse.cu, nvcc) and the host entry points (g++ -ffp-contract=off).  Every product and sum is one explicit rounding, so the device contracts nothing the
 // host does not.
 //
 // The reference evaluates cv::Mat expressions on CV_32F data.  What each one does, and how it is written here:
 //   p3Dc = Rcw*p3Dw + tcw          cv::gemm's small-matrix path: f32 products summed left to right, then + t (map_update_math.cuh)
-//   invz = 1/z, u = fx*x + cx      f32, left to right
+//   invz = 1/z, u = fx*x + cx      f32, left to right.  Fuse(Scw) writes 1.0/z: an f64 quotient rounded to f32, which equals the f32
+//                                  quotient (double rounding of a division is innocuous when 53 >= 2*24 + 2)
 //   IsInImage                      mnMinX <= u < mnMaxX, mnMinY <= v < mnMaxY
 //   1.2f*mfMaxDistance, 0.8f*mfMinDistance   GetMaxDistanceInvariance / GetMinDistanceInvariance, f32
 //   dist3D = cv::norm(p3Dw - Ow)   f32 difference, squares summed in double, sqrt, rounded to float (normal_depth_math.cuh)
@@ -26,13 +28,14 @@ namespace fusenb {
 
 namespace np = ccm::newpts;
 
-constexpr float TH = 3.0f;   // Fuse's default radius factor (cslam/include/cslam/ORBmatcher.h), as SearchInNeighbors calls it
+constexpr float TH = 3.0f;      // Fuse's default radius factor (cslam/include/cslam/ORBmatcher.h), as SearchInNeighbors calls it
+constexpr float TH_SCW = 4.0f;  // the radius factor LoopFinder / MapMerger::SearchAndFuse pass to Fuse(Scw)
 constexpr int TH_LOW = 50;   // ORBmatcher::TH_LOW
 
 // one keyframe as the prelude reads it
 struct Cam {
   float T[12];                          // [Rcw | tcw], 3x4 row-major
-  float O[3];                           // GetCameraCenter()
+  float O[3];                           // GetCameraCenter(), or Fuse(Scw)'s Ow = -Rcw^T tcw
   float fx, fy, cx, cy;
   float min_x, min_y, max_x, max_y;     // mnMinX, mnMinY, mnMaxX, mnMaxY
   float log_scale;                      // mfLogScaleFactor
@@ -72,10 +75,10 @@ CCM_NP_HD bool level_bracket(float ratio, float log_scale, int nlevels, int* lev
 // the reference's own arithmetic for a flagged pair; host only
 inline int settle_level(float ratio, float log_scale, int nlevels) { return level_of_quotient(logf(ratio) / log_scale, nlevels); }
 
-// The gates of Fuse for point P (world position, normal, mfMaxDistance, mfMinDistance) against keyframe c.  PASS: u, v, radius and
+// The gates of Fuse for point P (world position, normal, mfMaxDistance, mfMinDistance) against keyframe c, radius factor th.  PASS: u, v, radius and
 // level are the query of GetFeaturesInArea.  FLAGGED: u, v and ratio are set, the level is the caller's to settle (radius then follows
 // from it).  REJECT: a gate failed.
-CCM_NP_HD int prelude(const Cam& c, const float* scale_factors, const float P[3], const float N[3], float max_d, float min_d, float& u, float& v,
+CCM_NP_HD int prelude(const Cam& c, const float* scale_factors, float th, const float P[3], const float N[3], float max_d, float min_d, float& u, float& v,
                       float& radius, int& level, float& ratio) {
   float pc[3];
 #pragma unroll
@@ -100,7 +103,7 @@ CCM_NP_HD int prelude(const Cam& c, const float* scale_factors, const float P[3]
   if (dot < np::dmul(0.5, (double)dist3D)) return REJECT;            // viewing angle within 60 degrees
   ratio = np::fdiv(max_d, dist3D);
   if (!level_bracket(ratio, c.log_scale, c.nlevels, &level)) return FLAGGED;
-  radius = np::fmul(TH, scale_factors[level]);
+  radius = np::fmul(th, scale_factors[level]);
   return PASS;
 }
 

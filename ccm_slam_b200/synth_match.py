@@ -583,3 +583,231 @@ def fuse_scene_from_arrays(z):
         kfs.append(kf)
     points = {k[len("points_"):]: z[k] for k in z.files if k.startswith("points_")}
     return dict(cur=kfs[0], targets=kfs[1:], points=points, cur_point=z["cur_point"], cand=z["cand"])
+
+
+# ---- the corrected keyframes and the loop points of LoopFinder / MapMerger::SearchAndFuse ------------------------------------
+def split_scw(S):
+    """Fuse(Scw)'s split (S/ORBmatcher.cpp:1004-1008) over the f32 4x4 Scw, rounded as its cv::Mat expressions round: scw = sqrt of the
+    f64 dot of row 0 of sRcw, rounded to f32; Rcw = sRcw/scw and tcw = t/scw each an f64 quotient rounded to f32; Ow = -Rcw^T tcw with
+    cv::gemm's f32 products summed left to right.  Returns (Tcw (3,4) f32, Ow (3,) f32)."""
+    S = np.asarray(S, np.float32)
+    d = 0.0
+    for c in range(3):
+        d += float(S[0, c]) * float(S[0, c])
+    scw = np.float32(np.sqrt(d))
+    R = (S[:3, :3].astype(np.float64) / np.float64(scw)).astype(np.float32)
+    t = (S[:3, 3].astype(np.float64) / np.float64(scw)).astype(np.float32)
+    return np.concatenate([R, t[:, None]], 1), _neg_rt_t(R, t)
+
+
+def _neg_rt_t(R, t):
+    """-R^T t as the reference computes it: (-R).t() * t, f32 products summed left to right"""
+    Ow = np.empty(3, np.float32)
+    for r in range(3):
+        s = np.float32(-R[0, r]) * t[0]
+        s = np.float32(s + np.float32(-R[1, r]) * t[1])
+        Ow[r] = np.float32(s + np.float32(-R[2, r]) * t[2])
+    return Ow
+
+
+def _libm_logf():
+    """glibc's logf, which PredictScale's log(float) is"""
+    import ctypes
+    f = ctypes.CDLL("libm.so.6").logf
+    f.restype = ctypes.c_float
+    f.argtypes = [ctypes.c_float]
+    return f
+
+
+def _sim3_of(R, t, s):
+    """g2o::Sim3(R, t, s) as qx qy qz qw tx ty tz s (f64)"""
+    from scipy.spatial.transform import Rotation
+    return np.concatenate([Rotation.from_matrix(R).as_quat(), t, [s]]).astype(np.float64)
+
+
+def _orb_levels():
+    """mvScaleFactors as ORBextractor builds them (each level the previous times 1.2f), mvInvLevelSigma2 and mfLogScaleFactor"""
+    sf = np.empty(8, np.float32); sf[0] = 1
+    for i in range(1, 8):
+        sf[i] = np.float32(sf[i - 1] * np.float32(1.2))
+    return sf, (np.float32(1) / (sf * sf)).astype(np.float32), np.float32(np.log(np.float32(1.2)))
+
+
+def make_search_and_fuse_scene(kind="loop", n_kf=6, n=500, n_loop=None, seed=0, held_frac=0.1, occupied_frac=0.4, dup=20, bad_frac=0.03,
+                               dnr_frac=0.03, behind=8, outside=8, off_cone=8, boundary=24, far_frac=0.05, camera_probe=16):
+    """The corrected keyframes of a loop closure (kind "loop", s = 1) or a map merge (kind "merge", s != 1 per keyframe) and the loop
+    points vpLoopMapPoints, all looking at one seeded cloud.  Each keyframe's features are projections of the cloud through its pose plus
+    pixel noise, octaves follow depth, descriptors a per-point base with bits flipped.  The corrected Sim3 of keyframe k is
+    Scw = Sim3(R, s*t, s) of its pose [R | t]; its ccm_fuse_kf camera (Tcw, Ow) is Fuse(Scw)'s split of the f32 Scw (split_scw), and
+    Tcw_pose / Ow_pose hold the [R t/s] pose the keyframe itself stores, which differs from the split in rounding; sim3 is the g2o Sim3
+    itself (qx qy qz qw tx ty tz s).
+    The loop points (one row each in `points`) and the knobs:
+      held_frac       a keyframe's feature on a loop point's cloud point holds that very loop point (in spAlreadyFound)
+      occupied_frac   ... or holds a point of its own (kf_slot -2: an occupant that Replace would merge)
+      dup             pairs of loop points on one cloud point: both claim the same keypoint
+      bad_frac        points already bad (skip = 1); dnr_frac  points with mbDoNotReplace (dnr = 1, searched all the same)
+      behind / outside / off_cone   points behind the cameras, projecting outside the image, or with the normal turned away
+      boundary        points whose mfMaxDistance / dist3D sits within a few ulps of 1.2^k for keyframe 0's split centre: PredictScale's
+                      level hangs on the last bit of logf
+      far_frac        features placed 3.1 to 3.9 scale units from their projection (found with th = 4 only, and only without the
+                      chi-square gate of Fuse(kf, points))
+      camera_probe    points on keyframe 0 whose PredictScale level differs between the split centre and the [R t/s] pose's centre,
+                      at a level where their keypoint is searched under one of the two only
+    Returns dict(kind, kfs, points (pos, normal, max_d, min_d, desc, skip, dnr, world), kf_slot (per keyframe, per feature: the loop
+    row held, -2 an occupant, -1 empty), boundary_rows)."""
+    rng = np.random.default_rng(seed)
+    f = np.float32
+    n_loop = int(n_loop or 3 * n)
+    intr = (f(458.654), f(457.296), f(367.215), f(248.375))
+    W, H = 752, 480
+    sf, ils2, lsf = _orb_levels()
+    P0 = int(n_loop * 1.1)
+    X = np.stack([rng.uniform(-5, 5, P0), rng.uniform(-3.2, 3.2, P0), rng.uniform(4.0, 12.0, P0)], 1).astype(f)
+    base_desc = rng.integers(0, 256, size=(P0, 32), dtype=np.uint8)
+    d_ref = np.linalg.norm(X.astype(np.float64), axis=1)
+    l0 = rng.integers(0, 4, P0)
+    maxd = (d_ref * sf[l0]).astype(f)
+    mind = (maxd / sf[7]).astype(f)
+
+    def unit(v):
+        v = np.asarray(v, np.float64)
+        return (v / np.linalg.norm(v)).astype(f)
+
+    # the loop points: most of the cloud, a few twice (dup), then the knob points
+    world = list(rng.permutation(P0)[:n_loop - dup - behind - outside - off_cone - boundary])
+    world += [int(w) for w in rng.choice(world, size=dup, replace=False)]
+    m = len(world)
+    pts = dict(pos=(X[world] + rng.normal(0, 0.002, (m, 3))).astype(f), normal=np.stack([unit(X[w]) for w in world]).astype(f),
+               max_d=maxd[world].copy(), min_d=mind[world].copy(), desc=flip_bits(base_desc[world], rng.integers(0, 10, m), rng))
+    kfs = []
+    for k in range(n_kf):
+        c = rng.normal(0, 1, 3); c[2] *= 0.4
+        c = c / np.linalg.norm(c) * rng.uniform(0.2, 1.0)
+        R = _rot(rng.normal(0, 0.04, 3))
+        t = -R @ c
+        s = 1.0 if kind == "loop" else float(rng.uniform(0.6, 1.6))
+        S = np.eye(4); S[:3, :3] = s * R; S[:3, 3] = s * t
+        S = S.astype(f)                                                         # Converter::toCvMat(g2oScw)
+        Tcw, Ow = split_scw(S)
+        Rp = R.astype(f); tp = (s * t / s).astype(f)                            # the keyframe's pose [R t/s]
+        Xc = X.astype(np.float64) @ R.T + t
+        z = Xc[:, 2]
+        u = intr[0] * Xc[:, 0] / z + intr[2]
+        v = intr[1] * Xc[:, 1] / z + intr[3]
+        vis = np.flatnonzero((z > 0.5) & (u > 0) & (u < W) & (v > 0) & (v < H) & (rng.random(P0) < 0.85))
+        vis = rng.permutation(vis)[: n - n // 8]
+        mv = len(vis)
+        xy = np.stack([u[vis], v[vis]], 1) + rng.normal(0, 0.5, (mv, 2))
+        dist = fuse_dist3d(X[vis], Ow).astype(np.float64)
+        octave = np.clip(np.ceil(np.log(maxd[vis] / dist) / np.log(1.2)), 0, 7).astype(np.int64)
+        octave = np.where(rng.random(mv) < 0.2, np.maximum(octave - 1, 0), octave)
+        far = rng.random(mv) < far_frac                 # 3 to 4 radii out: inside th = 4, outside th = 3 and the chi-square gate
+        xy[far, 0] += rng.choice([-1, 1], far.sum()) * rng.uniform(3.1, 3.9, far.sum()) * sf[octave[far]]
+        desc = flip_bits(base_desc[vis], rng.integers(0, 20, mv), rng)
+        r = n - mv
+        kfs.append(dict(desc=np.concatenate([desc, rng.integers(0, 256, (r, 32), dtype=np.uint8)]),
+                        kp_xy=np.concatenate([xy, rng.uniform([0, 0], [W, H], (r, 2))]).astype(f),
+                        octave=np.concatenate([octave, rng.integers(0, 8, r)]).astype(np.int32), angle=np.zeros(n, f), bounds=(0, 0, W, H),
+                        cols=64, rows=48, intr=intr, sim3=_sim3_of(R, s * t, s), Scw=S, Tcw=Tcw, Ow=Ow, Tcw_pose=np.concatenate([Rp, tp[:, None]], 1),
+                        Ow_pose=_neg_rt_t(Rp, tp), scale_factors=sf.copy(), inv_level_sigma2=ils2.copy(), log_scale_factor=lsf,
+                        world=np.concatenate([vis, np.full(r, -1)])))
+    # the knob points
+    seen = [int(w) for w in kfs[0]["world"] if w >= 0]
+    knobs = dict(pos=[], normal=[], max_d=[], min_d=[], desc=[], world=[])
+
+    def knob(x, nrm, mx, mn, w):
+        knobs["pos"].append(np.asarray(x, f)); knobs["normal"].append(np.asarray(nrm, f)); knobs["max_d"].append(f(mx))
+        knobs["min_d"].append(f(mn)); knobs["desc"].append(base_desc[w]); knobs["world"].append(w)
+    for _ in range(behind):
+        w = seen[rng.integers(len(seen))]
+        knob(X[w] * f(-1.0), unit(X[w] * -1.0), maxd[w], mind[w], w)
+    for _ in range(outside):
+        w = seen[rng.integers(len(seen))]
+        x = X[w] + np.array([rng.choice([-1, 1]) * 40.0, 0, 0], f)
+        knob(x, unit(x), maxd[w] * 4, mind[w], w)
+    for _ in range(off_cone):
+        w = seen[rng.integers(len(seen))]
+        knob(X[w], -unit(X[w]), maxd[w], mind[w], w)
+    Ow0 = kfs[0]["Ow"]
+    for _ in range(boundary):
+        w = seen[rng.integers(len(seen))]
+        d = fuse_dist3d(X[w], Ow0)
+        mx = np.float32(np.float64(d) * 1.2 ** int(rng.integers(1, 5)))
+        off = int(rng.integers(0, 9)) - 4                           # a few ulps either side of the boundary
+        for _ in range(abs(off)):
+            mx = np.nextafter(mx, np.float32(np.inf if off > 0 else -np.inf), dtype=np.float32)
+        knob(X[w], unit(X[w] - Ow0), mx, mx / sf[7], w)
+    logf = _libm_logf()
+    j_of = {int(w): j for j, w in enumerate(kfs[0]["world"]) if w >= 0}
+    made = 0
+    for w in rng.permutation(seen):
+        if made >= camera_probe:
+            break
+        x = X[w]
+        ds, dp = fuse_dist3d(x, Ow0), fuse_dist3d(x, kfs[0]["Ow_pose"])
+        if ds == dp:
+            continue
+        o = int(kfs[0]["octave"][j_of[int(w)]])
+        if o > 5:
+            continue
+        mx = np.float32(np.float64(ds) * 1.2 ** (o + 1))
+        mx = np.nextafter(mx, np.float32(-np.inf), dtype=np.float32)
+        for _ in range(24):
+            mx = np.nextafter(mx, np.float32(np.inf), dtype=np.float32)
+            ls = int(np.ceil(np.float32(logf(np.float32(mx / ds)) / lsf)))
+            lp = int(np.ceil(np.float32(logf(np.float32(mx / dp)) / lsf)))
+            if ls != lp:
+                knob(x, unit(x - Ow0), mx, mx / sf[7], w)
+                made += 1
+                break
+    for key in ("pos", "normal", "max_d", "min_d", "desc"):
+        pts[key] = np.concatenate([pts[key], np.asarray(knobs[key]).reshape((-1,) + pts[key].shape[1:]).astype(pts[key].dtype)])
+    pts["world"] = np.asarray(world + knobs["world"], np.int64)
+    P = len(pts["world"])
+    boundary_rows = np.arange(P - boundary - made, P - made)
+    flag = rng.random(P)
+    pts["skip"] = (flag < bad_frac).astype(np.uint8)
+    pts["dnr"] = ((flag >= bad_frac) & (flag < bad_frac + dnr_frac)).astype(np.uint8)
+    # what each keyframe holds: a loop point on the feature's cloud point, an occupant of its own, or nothing
+    row_of = {}
+    for i, w in enumerate(world):
+        row_of.setdefault(int(w), i)
+    kf_slot = []
+    for kf in kfs:
+        sl = np.full(n, -1, np.int32)
+        for j, w in enumerate(kf["world"]):
+            a = rng.random()
+            if w >= 0 and int(w) in row_of and a < held_frac:
+                sl[j] = row_of[int(w)]
+            elif a < held_frac + occupied_frac:
+                sl[j] = -2
+        kf_slot.append(sl)
+    return dict(kind=kind, kfs=kfs, points=pts, kf_slot=kf_slot, boundary_rows=boundary_rows)
+
+
+_SF_KF_KEYS = ("desc", "kp_xy", "octave", "angle", "bounds", "cols", "rows", "intr", "Scw", "Tcw", "Ow", "Tcw_pose", "Ow_pose", "scale_factors",
+               "inv_level_sigma2", "log_scale_factor")
+
+
+def search_and_fuse_scene_arrays(sc):
+    """The parts of a make_search_and_fuse_scene dict that api.search_and_fuse reads, as flat named arrays (np.savez)"""
+    out = dict(n_kf=np.int64(len(sc["kfs"])))
+    for k, v in sc["points"].items():
+        out["points_" + k] = np.asarray(v)
+    for i, kf in enumerate(sc["kfs"]):
+        for k in _SF_KF_KEYS:
+            out["kf%d_%s" % (i, k)] = np.asarray(kf[k])
+    return out
+
+
+def search_and_fuse_scene_from_arrays(z):
+    """inverse of search_and_fuse_scene_arrays"""
+    kfs = []
+    for i in range(int(z["n_kf"])):
+        kf = {k: z["kf%d_%s" % (i, k)] for k in _SF_KF_KEYS}
+        kf["bounds"] = tuple(float(b) for b in kf["bounds"])
+        kf["cols"], kf["rows"] = int(kf["cols"]), int(kf["rows"])
+        kf["log_scale_factor"] = np.float32(kf["log_scale_factor"])
+        kfs.append(kf)
+    points = {k[len("points_"):]: z[k] for k in z.files if k.startswith("points_")}
+    return dict(kfs=kfs, points=points)

@@ -843,7 +843,7 @@ typedef struct ccm_fuse_points {      /* the map points the call may search, one
   const float* max_distance;          /* n   mfMaxDistance (the member's gate uses 1.2f times it, PredictScale the value itself) */
   const float* min_distance;          /* n   mfMinDistance */
   const uint8_t* desc;                /* n*32 GetDescriptor() */
-  const uint8_t* skip;                /* n   mbDoNotReplace || isBad() */
+  const uint8_t* skip;                /* n   ccm_fuse_neighbours: mbDoNotReplace || isBad();  ccm_search_and_fuse: isBad() only */
 } ccm_fuse_points;
 
 int ccm_fuse_neighbours(const ccm_fuse_kf* cur, const ccm_fuse_kf* targets, int32_t n_targets, const ccm_fuse_points* pts,
@@ -852,6 +852,37 @@ int ccm_fuse_neighbours(const ccm_fuse_kf* cur, const ccm_fuse_kf* targets, int3
 int ccm_fuse_neighbours_host(const ccm_fuse_kf* cur, const ccm_fuse_kf* targets, int32_t n_targets, const ccm_fuse_points* pts,
                              const int32_t* cur_point, const int32_t* cand, int32_t n_cand, int32_t* fwd_best, int32_t* bwd_best,
                              int32_t* n_settled);
+
+/* ---- loop and merge fusion -----------------------------------------------------------------------------------------------
+ * The searches of LoopFinder::SearchAndFuse (cslam/src/LoopFinder.cpp:709-734) and MapMerger::SearchAndFuse
+ * (cslam/src/MapMerger.cpp:574-598) in one call.  Both members run ORBmatcher::Fuse(pKF, Scw, vpLoopMapPoints, 4, vpReplacePoints)
+ * (cslam/src/ORBmatcher.cpp:995-1122) for each corrected keyframe in map order, then Replace / ReplaceAndLock each point the search
+ * found an occupant for.  The walk, the skip of points in pKF->GetMapPoints() and all map surgery stay with the caller.
+ *
+ * Why one pass is enough: a pair's search reads the point's position, normal, distance limits and descriptor, and the keyframe's
+ * keypoints, grid and Scw.  Of these only the descriptor changes during the member (Replace and ReplaceAndLock end with
+ * ComputeDistinctiveDescriptors on the survivor; nothing calls UpdateNormalAndDepth).  isBad() and GetMapPoints() change too, and
+ * the caller checks them live.  So every pair is searched here over the state at the start of the member, and the caller searches
+ * again (ccm_search_and_fuse_host, one keyframe) only points whose descriptor no longer equals the bytes passed in.
+ *
+ * Each (keyframe, point) pair runs Fuse(Scw)'s prelude (projection, IsInImage, the distance-invariance range, the 60-degree cone,
+ * PredictScale; ccm_slam_b200/csrc/fuse_neighbours_math.cuh) with th = 4 and its window search: levels [L-1, L], no chi-square
+ * gate, the first minimum of the Hamming distance, kept when <= TH_LOW.  mbDoNotReplace is not read (the reference comments it out).
+ * A pair whose PredictScale level depends on the last bit of logf is settled on the host with logf before the call returns
+ * (DESIGN.md §5); *n_settled (may be NULL) counts those pairs.
+ *
+ * In:  kfs[0..n_kf)   the corrected keyframes.  Tcw / Ow are the caller's split of the corrected Scw (Fuse's :1004-1008: scw = the
+ *                     norm of row 0 of sR, Rcw = sR/scw, tcw = t/scw, Ow = -Rcw^T tcw), not the keyframe's pose.  inv_level_sigma2
+ *                     is not read;
+ *      pts            the loop points vpLoopMapPoints, one row each; skip = isBad() on entry.
+ * Out: best[k * pts->n + i]   keypoint of keyframe k that loop point i lands on, or -1.
+ * A null array, a grid with more keypoints than the 20-bit visiting position of the window key holds, or more than 2^30 pairs
+ * (each keyframe's points padded to a multiple of 32) fails with CCM_ERR_INVALID and a message naming the keyframe; nothing is
+ * written.  No pairs: no launch.
+ * ccm_search_and_fuse: one upload, one launch whatever n_kf, one download; no atomics, identical bytes every call.
+ * ccm_search_and_fuse_host: the same contract without a device; the two agree bit for bit. */
+int ccm_search_and_fuse(const ccm_fuse_kf* kfs, int32_t n_kf, const ccm_fuse_points* pts, int32_t* best, int32_t* n_settled);
+int ccm_search_and_fuse_host(const ccm_fuse_kf* kfs, int32_t n_kf, const ccm_fuse_points* pts, int32_t* best, int32_t* n_settled);
 
 /* ---- Sim3 correction of a loop closure or a map merge ---------------------------------------------------------------------
  * The pass over CorrectedSim3 of LoopFinder::CorrectLoop (cslam/src/LoopFinder.cpp:568-613) and over CorrectedSim3All of
