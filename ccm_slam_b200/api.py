@@ -261,6 +261,16 @@ class BAHandle:
         _chk(lib().ccm_ba_debug_schur(self._h, int(robust), C.c_double(huber_delta), C.c_double(lam), _p(S), _p(bs), _p(dxp), _p(dxl), C.byref(it), C.byref(rr)))
         return dict(S=S, bschur=bs, dx_pose=dxp, dx_point=dxl, pcg_iters=it.value, pcg_relres=rr.value)
 
+    def debug_step(self, dx_pose, lam, robust=True, huber_delta=HUBER_GBA):
+        """one LM trial from the given pose step x (K, 6) at damping lam, without the Schur and PCG passes: the trial state, the landmark
+        step, the trial robust chi2 and the pose / landmark halves of the gain-ratio denominator (ccm_ba_debug_step)"""
+        x = np.ascontiguousarray(dx_pose, np.float64).reshape(self.K, 6)
+        pose = np.empty((self.K, 7)); pt = np.empty((self.P, 3)); dxl = np.empty((self.P, 3))
+        chi, sp, sl = C.c_double(), C.c_double(), C.c_double()
+        _chk(lib().ccm_ba_debug_step(self._h, int(robust), C.c_double(huber_delta), C.c_double(lam), _p(x), _p(pose), _p(pt), _p(dxl),
+                                     C.byref(chi), C.byref(sp), C.byref(sl)))
+        return dict(pose_trial=pose, pt_trial=pt, dx_point=dxl, chi2_trial=chi.value, scale_pose=sp.value, scale_point=sl.value)
+
     def debug_schur_blocks(self):
         """S and b_schur as the last debug_schur left them: block CSR in pose indices (rowptr (K+1,), col (nnzb,), val (nnzb,6,6)),
         fixed poses with empty rows, and b_schur (K,6)."""

@@ -68,6 +68,18 @@ __global__ void __launch_bounds__(TPB) k_lin_heads(const int* __restrict__ lm_pt
   head[l] = h;
 }
 
+// An inactive edge (weight 0: g2o's level 1, which g2o never evaluates) must contribute exact zeros, also where its point sits at
+// depth 0 and its projection is not finite (0 * inf = NaN).  Its linearisation runs like any other, without a divergent branch, and
+// is then replaced by zeros; an active edge's values pass through unchanged.
+__device__ __forceinline__ void drop_inactive(double w, ObsLin& L) {
+  const bool on = w != 0.0;
+  L.ex = on ? L.ex : 0.0; L.ey = on ? L.ey : 0.0; L.chi2 = on ? L.chi2 : 0.0;
+#pragma unroll
+  for (int i = 0; i < 6; i++) L.Jl[i] = on ? L.Jl[i] : 0.0;
+#pragma unroll
+  for (int i = 0; i < 12; i++) L.Jp[i] = on ? L.Jp[i] : 0.0;
+}
+
 // K1+K2 of one observation for the thread's slot t of the chunk [c0, c1): the 6x3 W row into s_w (row stride 19), and with
 // hsum the 9 point-side terms (Hll upper, bl) into s_h and the robust chi2 into chi.  dbgW (debug export only): W as
 // [18][Ep] SoA.  Returns the observation's landmark (-1 past the chunk).
@@ -91,6 +103,7 @@ __device__ __forceinline__ int lin_obs(int c0, int c1, const int* __restrict__ o
   const double* X = pt + 3 * (size_t)lm;
   ObsLin L;
   linearize_obs(T, in4, X[0], X[1], X[2], (double)uv.x, (double)uv.y, w, L);
+  drop_inactive(w, L);
   double rho0 = L.chi2, rho1 = 1.0;
   if (rob) huber(L.chi2, delta, rho0, rho1);
   const double wo = rho1 * w;                     // weightedOmega = rho'(chi2) * omega
@@ -242,7 +255,7 @@ __global__ void __launch_bounds__(TPB) k_residual(
     project_residual(T, in4, X[0], X[1], X[2], (double)uv.x, (double)uv.y, w, ex, ey, chi2, Xc);
     double rho0 = chi2, rho1;
     if (robust && !signbit(wf)) huber(chi2, delta, rho0, rho1);
-    chi_acc += rho0;
+    chi_acc += w != 0.0 ? rho0 : 0.0;   // an inactive edge adds nothing, even where its chi2 is not finite (drop_inactive)
   }
   const double tot = block_sum(chi_acc, red);
   if (threadIdx.x == 0) chi2_partials[blockIdx.x] = tot;
@@ -313,6 +326,7 @@ __global__ void __launch_bounds__(128) k_pose_pass(
     const double* X = pt + 3 * (size_t)lm;
     ObsLin L;
     linearize_obs(T, in4, X[0], X[1], X[2], (double)ob.x, (double)ob.y, w, L);
+    drop_inactive(w, L);
     double rho0, rho1 = 1.0;
     if (robust && !signbit(wf)) huber(L.chi2, delta, rho0, rho1);
     const double wo = rho1 * w;

@@ -1260,6 +1260,37 @@ extern "C" int ccm_ba_debug_schur(ccm_ba_handle* h, int robust, double huber_del
   });
 }
 
+extern "C" int ccm_ba_debug_step(ccm_ba_handle* h, int robust, double huber_delta, double lambda, const double* dx_pose,
+                                 double* pose_trial, double* pt_trial, double* dx_point, double* chi2_trial, double* scale_pose,
+                                 double* scale_point) {
+  return guarded([&] {
+    CCM_REQUIRE(h && dx_pose, "null argument");
+    CCM_REQUIRE(h->nranks == 1, "debug entry points are single-rank");
+    CCM_CUDA(cudaSetDevice(h->device));
+    cudaStream_t s = h->stream;
+    const int K = h->K, Kf = h->Kf, Pl = h->Pl;
+    std::vector<double> hx((size_t)std::max(Kf, 1) * 6, 0.0);
+    for (int a = 0; a < Kf; a++) memcpy(hx.data() + (size_t)a * 6, dx_pose + 6 * (size_t)h->h_slot_pose[a], 6 * sizeof(double));
+    step_linearize(h, robust, huber_delta, LIN_Z, lambda);
+    if (Kf > 0) h->x.upload(hx.data(), (size_t)Kf * 6, s);
+    step_update_and_residual(h, lambda, robust, huber_delta, h->dxl.p);
+    std::vector<double> hp((size_t)K * 7), hq((size_t)Pl * 3), hd((size_t)Pl * 3), sc(3);
+    if (K > 0) CCM_CUDA(cudaMemcpyAsync(hp.data(), h->pose_trial, hp.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+    if (Pl > 0) {
+      CCM_CUDA(cudaMemcpyAsync(hq.data(), h->pt_trial, hq.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+      h->dxl.download(hd.data(), hd.size(), s);
+    }
+    h->scal.download(sc.data(), 3, s);
+    CCM_CUDA(cudaStreamSynchronize(s));
+    if (pose_trial) memcpy(pose_trial, hp.data(), hp.size() * sizeof(double));
+    if (pt_trial) memcpy(pt_trial, hq.data(), hq.size() * sizeof(double));
+    if (dx_point) memcpy(dx_point, hd.data(), hd.size() * sizeof(double));
+    if (chi2_trial) *chi2_trial = sc[0];
+    if (scale_point) *scale_point = sc[1];
+    if (scale_pose) *scale_pose = sc[2];
+  });
+}
+
 extern "C" int ccm_ba_debug_schur_blocks(ccm_ba_handle* h, int32_t* rowptr, int32_t* col, double* val, double* bschur) {
   return guarded([&] {
     CCM_REQUIRE(h, "null handle");

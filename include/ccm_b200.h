@@ -168,6 +168,13 @@ int ccm_ba_debug_build(ccm_ba_handle* h, int robust, double huber_delta,
 int ccm_ba_debug_schur(ccm_ba_handle* h, int robust, double huber_delta, double lambda,
                        double* S_dense /*(6K)^2 or NULL*/, double* bschur /*6K or NULL*/,
                        double* dx_pose /*K*6*/, double* dx_point /*P*3*/, int32_t* pcg_iters, double* pcg_relres);
+/* one LM trial from a caller-given pose step, without the Schur and PCG passes: linearise at the current estimate with damping
+ * lambda, then the pose update exp(x) * T, the landmark back-substitution from x, and the robust chi2 of the trial state.
+ * dx_pose (K*6, caller's pose indices; rows of fixed poses are ignored) is x.  Outputs: the trial state, the landmark step, the trial
+ * chi2 and the two halves of the gain-ratio denominator, sum x (lambda x + bp) and sum xl (lambda xl + bl).  Any output may be NULL. */
+int ccm_ba_debug_step(ccm_ba_handle* h, int robust, double huber_delta, double lambda, const double* dx_pose /*K*6*/,
+                      double* pose_trial /*K*7*/, double* pt_trial /*P*3*/, double* dx_point /*P*3*/, double* chi2_trial,
+                      double* scale_pose, double* scale_point);
 /* S (lambda included) and b_schur as the last ccm_ba_debug_schur left them, as block CSR in the caller's pose indices: every stored
  * 6x6 block of the full symmetric pattern, row-major, columns ascending; fixed poses have empty rows and zero b_schur.
  * nnzb = ccm_ba_info.s_blocks_full.  Any output may be NULL. */
