@@ -3,10 +3,12 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <algorithm>
 #include <atomic>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <exception>
 #include <stdexcept>
 #include <string>
 #include <vector>
@@ -58,7 +60,11 @@ struct DevBuf {
   DevBuf() = default;
   DevBuf(const DevBuf&) = delete;
   DevBuf& operator=(const DevBuf&) = delete;
-  ~DevBuf() { release(); }
+  ~DevBuf() {
+    // on an error path work queued on the caller's stream may still use the block: dev_free's contract wants it finished
+    if (p && std::uncaught_exceptions()) cudaDeviceSynchronize();
+    release();
+  }
   void release() {
     if (p) dev_free(p);
     p = nullptr; n = 0;
@@ -84,7 +90,21 @@ struct DevBuf {
 
 inline int div_up(long long a, long long b) { return (int)((a + b - 1) / b); }
 
-// Lays arrays out in one block at 16-byte boundaries, for a single upload (new_points.cu, fuse_neighbours.cu).  Without a host block it
+int sm_count();
+
+// blocks for n items at per_cta items a block, at most eight per SM (the kernels loop over the rest), at least one
+inline int grid_size(long long n, int per_cta) { return std::max(1, std::min(div_up(n, per_cta), sm_count() * 8)); }
+
+// a non-blocking stream for the length of one call
+struct CallStream {
+  cudaStream_t s = nullptr;
+  CallStream() { CCM_CUDA(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking)); }
+  CallStream(const CallStream&) = delete;
+  CallStream& operator=(const CallStream&) = delete;
+  ~CallStream() { cudaStreamDestroy(s); }
+};
+
+// Lays arrays out in one block at 16-byte boundaries, for a single upload (Staging::upload).  Without a host block it
 // only measures; with one it copies each array in and answers the address the array will have on the device.
 struct Packer {
   size_t at = 0;
@@ -104,8 +124,53 @@ struct Packer {
   }
 };
 
+// The staging of one batched entry point, which keeps its own thread_local instance: a stream, a pinned block and a device block each
+// way.  A block too small for a call grows to 1.25x what the call needs.  The stream and the device blocks belong to the device they
+// were made on: the first call after ccm_init picks another device releases them.  The pinned output holds a call's results until the
+// thread's next call that uses the same instance.
+struct Staging {
+  cudaStream_t stream = nullptr;
+  int device = -1;
+  uint8_t* h_in = nullptr;
+  uint8_t* h_out = nullptr;
+  size_t h_in_cap = 0, h_out_cap = 0;
+  DevBuf<uint8_t> in, out;
+  Staging() = default;
+  Staging(const Staging&) = delete;
+  Staging& operator=(const Staging&) = delete;
+  ~Staging();
+  // blocks of at least these sizes in bytes: device input, device output, pinned input, pinned output
+  void reserve(size_t d_in, size_t d_out, size_t p_in, size_t p_out);
+  // pack(Packer&) lays the upload out; it runs twice, to measure and then to fill the pinned input.  The device output grows to
+  // out_bytes, of which the first down_bytes come back through the pinned output.  Queues the upload on `stream`.
+  template <typename F>
+  void upload(F&& pack, size_t out_bytes, size_t down_bytes) {
+    Packer measure;
+    pack(measure);
+    const size_t bytes = measure.at;
+    reserve(bytes, out_bytes, bytes, down_bytes);
+    Packer pk;
+    pk.host = h_in; pk.dev = in.p;
+    pack(pk);
+    CCM_CUDA(cudaMemcpyAsync(in.p, h_in, bytes, cudaMemcpyHostToDevice, stream));
+  }
+  // runs a call's device work, f(), on the current device's stream; if f throws, the stream is drained before the exception leaves,
+  // so no copy of the call still reads the pinned blocks or writes the caller's arrays
+  template <typename F>
+  void run(F&& f) {
+    use_current_device();
+    struct Drain {
+      cudaStream_t s;
+      ~Drain() { if (std::uncaught_exceptions()) cudaStreamSynchronize(s); }
+    } drain{stream};
+    f();
+  }
+
+ private:
+  void use_current_device();
+};
+
 int current_device();      // device chosen by ccm_init (default 0)
-int sm_count();
 void ensure_device();      // throws CCM_ERR_NO_DEVICE when there is none
 
 // ---- NCCL communicator (dlopen'ed) ----

@@ -272,11 +272,6 @@ std::string row_error(const std::string& f, int32_t b, int32_t n_kf, const uint6
   return "";
 }
 
-struct StreamGuard {
-  cudaStream_t s = nullptr;
-  ~StreamGuard() { if (s) cudaStreamDestroy(s); }
-};
-
 }  // namespace
 
 extern "C" int ccm_covisibility_host(int32_t n_kf, const uint64_t* kf_id, const uint32_t* kf_rank, int32_t n_b, const int32_t* batch,
@@ -348,8 +343,7 @@ extern "C" int ccm_covisibility(int32_t n_kf, const uint64_t* kf_id, const uint3
     ensure_device();
     if (n_b == 0) { *total = 0; conn_ptr[0] = 0; return; }
     const int64_t M = kf_mp_ptr[n_b], E = n_mp ? obs_ptr[n_mp] : 0;
-    StreamGuard g;
-    CCM_CUDA(cudaStreamCreateWithFlags(&g.s, cudaStreamNonBlocking));
+    const CallStream g;
     std::vector<int32_t> inv(std::max(n_kf, 1), 0);
     for (int32_t k = 0; k < n_kf; k++) inv[kf_rank[k]] = k;
     DevBuf<uint64_t> d_id;

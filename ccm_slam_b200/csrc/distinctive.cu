@@ -296,11 +296,11 @@ void run_device(const std::string& f, cudaStream_t s, int32_t n_kf, const uint8_
   CCM_CUDA(cudaMemsetAsync(d_counts.p, 0, 3 * sizeof(int32_t), s));
   CCM_CUDA(cudaMemsetAsync(d_counts.p + 3, 0x7f, sizeof(int32_t), s));
   const int sms = sm_count();
-  k_dd_classify<<<std::min(div_up(n_mp, CTA), sms * 8), CTA, 0, s>>>(n_mp, n_kf, d_bad.p, d_ptr.p, d_obs.p, src, d_nsurv.p, d_lists.p,
-                                                                      d_counts.p, d_counts.p + 3, d_best.p, d_med.p, d_desc.p);
+  k_dd_classify<<<grid_size(n_mp, CTA), CTA, 0, s>>>(n_mp, n_kf, d_bad.p, d_ptr.p, d_obs.p, src, d_nsurv.p, d_lists.p,
+                                                      d_counts.p, d_counts.p + 3, d_best.p, d_med.p, d_desc.p);
   CCM_LAUNCHED();
-  k_dd_warp<<<std::min(div_up(n_mp, CTA / 32), sms * 8), CTA, 0, s>>>(d_lists.p, d_counts.p, d_bad.p, d_ptr.p, d_obs.p, src, d_nsurv.p,
-                                                                      d_best.p, d_med.p, d_desc.p);
+  k_dd_warp<<<grid_size(n_mp, CTA / 32), CTA, 0, s>>>(d_lists.p, d_counts.p, d_bad.p, d_ptr.p, d_obs.p, src, d_nsurv.p,
+                                                      d_best.p, d_med.p, d_desc.p);
   CCM_LAUNCHED();
   k_dd_cta<<<std::min(n_mp, sms * 6), CTA, 0, s>>>(d_lists.p + n_mp, d_lists.p + 2 * (size_t)n_mp, d_counts.p, d_bad.p, d_ptr.p, d_obs.p, src,
                                                    d_nsurv.p, d_best.p, d_med.p, d_desc.p);
@@ -314,11 +314,6 @@ void run_device(const std::string& f, cudaStream_t s, int32_t n_kf, const uint8_
   if (desc_out) CCM_CUDA(cudaMemcpyAsync(desc_out, d_desc.p, (size_t)n_mp * 32, cudaMemcpyDeviceToHost, s));
   CCM_CUDA(cudaStreamSynchronize(s));
 }
-
-struct StreamGuard {
-  cudaStream_t s = nullptr;
-  ~StreamGuard() { if (s) cudaStreamDestroy(s); }
-};
 
 }  // namespace
 
@@ -381,8 +376,7 @@ extern "C" int ccm_distinctive_descriptors(int32_t n_kf, const uint8_t* kf_bad, 
     ensure_device();
     if (n_mp == 0) return;
     const int64_t E = obs_ptr[n_mp];
-    StreamGuard g;
-    CCM_CUDA(cudaStreamCreateWithFlags(&g.s, cudaStreamNonBlocking));
+    const CallStream g;
     DevBuf<uint8_t> d_bad;
     DevBuf<int64_t> d_ptr;
     DevBuf<int32_t> d_obs;
@@ -413,8 +407,7 @@ extern "C" int ccm_kfstore_distinctive_descriptors(ccm_kf_store* store, int32_t 
     kfstore_resolve(store, n_kf, kf_uid, base, n_feat, &device);
     CCM_CUDA(cudaSetDevice(device));
     const int64_t E = obs_ptr[n_mp];
-    StreamGuard g;
-    CCM_CUDA(cudaStreamCreateWithFlags(&g.s, cudaStreamNonBlocking));
+    const CallStream g;
     DevBuf<uint8_t> d_bad;
     DevBuf<int64_t> d_ptr;
     DevBuf<int32_t> d_obs, d_feat, d_nfeat;

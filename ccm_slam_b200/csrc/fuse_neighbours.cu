@@ -102,11 +102,11 @@ void scatter(const std::vector<int32_t>& out, long long n_fwd, int32_t* fwd_best
   if ((long long)out.size() > n_fwd) memcpy(bwd_best, out.data() + n_fwd, (out.size() - n_fwd) * sizeof(int32_t));
 }
 
-thread_local Scratch t_scr;
+thread_local Staging t_stage;
 
 // the Kf table (row 0 the current keyframe) followed by every array the kernel reads
-size_t pack(Packer& pk, const std::vector<HostKf>& kfs, const ccm_fuse_kf* cur, const ccm_fuse_kf* targets, const ccm_fuse_points* pts,
-            const int32_t* cur_point, const int32_t* cand, int32_t n_cand, Pts* dp, const int32_t** d_cur_point, const int32_t** d_cand) {
+void pack(Packer& pk, const std::vector<HostKf>& kfs, const ccm_fuse_kf* cur, const ccm_fuse_kf* targets, const ccm_fuse_points* pts,
+          const int32_t* cur_point, const int32_t* cand, int32_t n_cand, Pts* dp, const int32_t** d_cur_point, const int32_t** d_cand) {
   Kf* table = pk.host ? reinterpret_cast<Kf*>(pk.host + pk.at) : nullptr;
   pk.reserve(kfs.size() * sizeof(Kf));
   for (size_t r = 0; r < kfs.size(); r++) {
@@ -116,7 +116,6 @@ size_t pack(Packer& pk, const std::vector<HostKf>& kfs, const ccm_fuse_kf* cur, 
   *dp = put_points(pk, pts);
   *d_cur_point = pk.put(cur_point, (size_t)cur->grid.n);
   *d_cand = pk.put(cand, (size_t)n_cand);
-  return pk.at;
 }
 
 }  // namespace
@@ -149,27 +148,21 @@ extern "C" int ccm_fuse_neighbours(const ccm_fuse_kf* cur, const ccm_fuse_kf* ta
     if (n_pairs == 0) return;
     const std::vector<HostKf> kfs = host_kfs(cur, targets, n_targets);
 
-    Scratch& s = t_scr;
+    Staging& s = t_stage;
     Pts dp{};
     const int32_t *d_cur_point = nullptr, *d_cand = nullptr;
-    Packer measure;
-    const size_t bytes = pack(measure, kfs, cur, targets, pts, cur_point, cand, n_cand, &dp, &d_cur_point, &d_cand);
-    s.prepare(bytes, (size_t)n_pairs);
-    Packer pk;
-    pk.host = s.h_blob; pk.dev = s.blob.p;
-    pack(pk, kfs, cur, targets, pts, cur_point, cand, n_cand, &dp, &d_cur_point, &d_cand);
-    try {
-      CCM_CUDA(cudaMemcpyAsync(s.blob.p, s.h_blob, bytes, cudaMemcpyHostToDevice, s.stream));
-      k_fuse_pairs<<<div_up(n_pairs * 32, CTA), CTA, 0, s.stream>>>(reinterpret_cast<const Kf*>(s.blob.p), dp, d_cur_point, d_cand, n,
-                                                                     n_targets, (int)n_pairs, s.out.p);
+    const size_t out_bytes = (size_t)n_pairs * sizeof(int32_t);
+    s.run([&] {
+      s.upload([&](Packer& pk) { pack(pk, kfs, cur, targets, pts, cur_point, cand, n_cand, &dp, &d_cur_point, &d_cand); }, out_bytes, out_bytes);
+      int32_t* d_out = reinterpret_cast<int32_t*>(s.out.p);
+      k_fuse_pairs<<<div_up(n_pairs * 32, CTA), CTA, 0, s.stream>>>(reinterpret_cast<const Kf*>(s.in.p), dp, d_cur_point, d_cand, n,
+                                                                     n_targets, (int)n_pairs, d_out);
       CCM_LAUNCHED();
-      s.out.download(s.h_out, (size_t)n_pairs, s.stream);
+      CCM_CUDA(cudaMemcpyAsync(s.h_out, d_out, out_bytes, cudaMemcpyDeviceToHost, s.stream));
       CCM_CUDA(cudaStreamSynchronize(s.stream));
-    } catch (...) {
-      cudaStreamSynchronize(s.stream);   // nothing of this call may still read the pinned block
-      throw;
-    }
-    std::vector<int32_t> out(s.h_out, s.h_out + n_pairs);
+    });
+    const int32_t* h_out = reinterpret_cast<const int32_t*>(s.h_out);
+    std::vector<int32_t> out(h_out, h_out + n_pairs);
     int settled = 0;
     const HostPts hp(*pts);
     for (long long w = 0; w < n_pairs; w++) {

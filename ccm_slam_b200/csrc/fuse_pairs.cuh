@@ -139,46 +139,6 @@ inline void check_points(const std::string& f, const ccm_fuse_points* pts) {
               f + ": null point array");
 }
 
-// per-thread staging: one pinned block for the upload and one for the download, device blocks grown on demand
-struct Scratch {
-  cudaStream_t stream = nullptr;
-  int device = -1;
-  uint8_t* h_blob = nullptr;
-  size_t h_cap = 0;
-  int32_t* h_out = nullptr;
-  size_t h_out_cap = 0;
-  DevBuf<uint8_t> blob;
-  DevBuf<int32_t> out;
-  ~Scratch() {
-    if (h_blob) cudaFreeHost(h_blob);
-    if (h_out) cudaFreeHost(h_out);
-    if (stream) cudaStreamDestroy(stream);
-  }
-  // the stream and blocks of the current device, with room for `bytes` of upload and `n_out` results
-  void prepare(size_t bytes, size_t n_out) {
-    if (device != current_device()) {   // the blocks belong to the device they were allocated on
-      if (stream) { cudaStreamDestroy(stream); stream = nullptr; }
-      blob.release(); out.release();
-      device = current_device();
-    }
-    if (!stream) CCM_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
-    if (h_cap < bytes) {
-      if (h_blob) cudaFreeHost(h_blob);
-      h_blob = nullptr; h_cap = 0;
-      CCM_CUDA(cudaMallocHost((void**)&h_blob, bytes + bytes / 4));
-      h_cap = bytes + bytes / 4;
-    }
-    if (h_out_cap < n_out) {
-      if (h_out) cudaFreeHost(h_out);
-      h_out = nullptr; h_out_cap = 0;
-      CCM_CUDA(cudaMallocHost((void**)&h_out, (n_out + n_out / 4) * sizeof(int32_t)));
-      h_out_cap = n_out + n_out / 4;
-    }
-    if (blob.n < bytes) blob.alloc(bytes + bytes / 4);
-    if (out.n < n_out) out.alloc(n_out + n_out / 4);
-  }
-};
-
 // a keyframe's arrays into the upload block; returns its record with device addresses
 inline Kf put_kf(Packer& pk, const HostKf& h, const ccm_fuse_kf& f) {
   Kf k = h.k;

@@ -69,17 +69,16 @@ extern "C" int ccm_gba_map_update(int32_t n_kf, const int32_t* kf_parent, const 
     std::vector<float> twc((size_t)n_kf * 16, 0.f);
     for (int k = 0; k < n_kf; k++)
       if (kf_visited[k]) mu::pose_inverse(kf_TcwGBA + 16 * (size_t)k, twc.data() + 16 * (size_t)k);   // SetPose(mTcwGBA)
-    cudaStream_t s = nullptr;
-    CCM_CUDA(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
-    struct StreamGuard { cudaStream_t s; ~StreamGuard() { cudaStreamDestroy(s); } } guard{s};
+    const CallStream cs;
+    const cudaStream_t s = cs.s;
     DevBuf<uint8_t> d_state, d_vis, d_corr; DevBuf<int> d_ref; DevBuf<float> d_pos, d_gba, d_before, d_twc, d_out;
     d_state.upload(mp_state, n_mp, s); d_ref.upload(mp_ref, n_mp, s);
     d_pos.upload(mp_pos, (size_t)n_mp * 3, s); d_gba.upload(mp_pos_gba, (size_t)n_mp * 3, s);
     if (n_kf) { d_vis.upload(kf_visited, n_kf, s); d_before.upload(kf_Tcw, (size_t)n_kf * 16, s); d_twc.upload(twc.data(), twc.size(), s); }
     else { d_vis.alloc(1); d_before.alloc(16); d_twc.alloc(16); }
     d_out.alloc((size_t)n_mp * 3); d_corr.alloc(n_mp);
-    const int grid = std::min(div_up(n_mp, 256), sm_count() * 8);
-    k_map_update_points<<<grid, 256, 0, s>>>(n_mp, d_state.p, d_ref.p, d_pos.p, d_gba.p, d_vis.p, d_before.p, d_twc.p, d_out.p, d_corr.p);
+    k_map_update_points<<<grid_size(n_mp, 256), 256, 0, s>>>(n_mp, d_state.p, d_ref.p, d_pos.p, d_gba.p, d_vis.p, d_before.p, d_twc.p,
+                                                              d_out.p, d_corr.p);
     CCM_LAUNCHED();
     d_out.download(mp_pos_out, (size_t)n_mp * 3, s);
     d_corr.download(mp_corrected, n_mp, s);

@@ -42,49 +42,36 @@ __global__ void __launch_bounds__(256) k_hamming(const uint4* __restrict__ A, in
   }
 }
 
-// per-thread scratch: device buffers + pinned result, grown on demand (the matchers are called from several threads)
-struct Scratch {
-  cudaStream_t stream = nullptr;
-  int device = -1;
-  DevBuf<uint4> A, B;
-  DevBuf<uint16_t> D;
-  uint16_t* hD = nullptr;
-  size_t hD_cap = 0;
-  ~Scratch() {
-    if (hD) cudaFreeHost(hD);
-    if (stream) cudaStreamDestroy(stream);
-  }
-};
-thread_local Scratch t_scr;
+// per-thread staging (Staging; the matchers are called from several threads): the host operands go straight from the caller's memory
+// into the device input block, the distances come back through the pinned output block
+thread_local Staging t_stage;
 
 // Either operand may already live on the device (dA / dB != nullptr: the keyframe store of kf_store.cu); host operands are uploaded.
 const uint16_t* distance_matrix_any(const uint8_t* A, const uint4* dA, int nA, const uint8_t* B, const uint4* dB, int nB) {
   ensure_device();
-  Scratch& s = t_scr;
-  if (s.device != current_device()) {
-    if (s.stream) { cudaStreamDestroy(s.stream); s.stream = nullptr; }
-    s.device = current_device();
-  }
-  if (!s.stream) CCM_CUDA(cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking));
+  Staging& s = t_stage;
   const size_t n = (size_t)nA * nB;
-  if (n == 0) return s.hD;
-  if (!dA && s.A.n < (size_t)nA * 2) s.A.alloc((size_t)nA * 2 + 256);
-  if (!dB && s.B.n < (size_t)nB * 2) s.B.alloc((size_t)nB * 2 + 256);
-  if (s.D.n < n) s.D.alloc(n + 4096);
-  if (s.hD_cap < n) {
-    if (s.hD) cudaFreeHost(s.hD);
-    s.hD = nullptr;
-    CCM_CUDA(cudaMallocHost((void**)&s.hD, (n + 4096) * sizeof(uint16_t)));
-    s.hD_cap = n + 4096;
-  }
-  if (!dA) { CCM_CUDA(cudaMemcpyAsync(s.A.p, A, (size_t)nA * 32, cudaMemcpyHostToDevice, s.stream)); dA = s.A.p; }
-  if (!dB) { CCM_CUDA(cudaMemcpyAsync(s.B.p, B, (size_t)nB * 32, cudaMemcpyHostToDevice, s.stream)); dB = s.B.p; }
-  dim3 g(div_up(nB, 32), div_up(nA, 32));
-  k_hamming<<<g, 256, 0, s.stream>>>(dA, nA, dB, nB, s.D.p);
-  CCM_LAUNCHED();
-  CCM_CUDA(cudaMemcpyAsync(s.hD, s.D.p, n * sizeof(uint16_t), cudaMemcpyDeviceToHost, s.stream));
-  CCM_CUDA(cudaStreamSynchronize(s.stream));
-  return s.hD;
+  if (n == 0) return reinterpret_cast<const uint16_t*>(s.h_out);
+  Packer lay;
+  const size_t at_a = lay.reserve(dA ? 0 : (size_t)nA * 32), at_b = lay.reserve(dB ? 0 : (size_t)nB * 32);
+  s.run([&] {
+    s.reserve(lay.at, n * sizeof(uint16_t), 0, n * sizeof(uint16_t));
+    if (!dA) {
+      CCM_CUDA(cudaMemcpyAsync(s.in.p + at_a, A, (size_t)nA * 32, cudaMemcpyHostToDevice, s.stream));
+      dA = reinterpret_cast<const uint4*>(s.in.p + at_a);
+    }
+    if (!dB) {
+      CCM_CUDA(cudaMemcpyAsync(s.in.p + at_b, B, (size_t)nB * 32, cudaMemcpyHostToDevice, s.stream));
+      dB = reinterpret_cast<const uint4*>(s.in.p + at_b);
+    }
+    uint16_t* D = reinterpret_cast<uint16_t*>(s.out.p);
+    dim3 g(div_up(nB, 32), div_up(nA, 32));
+    k_hamming<<<g, 256, 0, s.stream>>>(dA, nA, dB, nB, D);
+    CCM_LAUNCHED();
+    CCM_CUDA(cudaMemcpyAsync(s.h_out, D, n * sizeof(uint16_t), cudaMemcpyDeviceToHost, s.stream));
+    CCM_CUDA(cudaStreamSynchronize(s.stream));
+  });
+  return reinterpret_cast<const uint16_t*>(s.h_out);
 }
 const uint16_t* distance_matrix(const uint8_t* A, int nA, const uint8_t* B, int nB) { return distance_matrix_any(A, nullptr, nA, B, nullptr, nB); }
 

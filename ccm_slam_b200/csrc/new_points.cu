@@ -260,28 +260,11 @@ void fill_empty(int64_t cells, int32_t* n_out, int32_t* best2, uint8_t* verdict)
   throw Error(CCM_ERR_INVALID, f + ": capacity " + std::to_string(capacity) + " below the " + std::to_string(needed) + " points needed");
 }
 
-// per-thread staging: one pinned block for the upload, device blocks grown on demand (LocalMapping calls once per keyframe)
-struct Scratch {
-  cudaStream_t stream = nullptr;
-  int device = -1;
-  uint8_t* h_blob = nullptr;
-  size_t h_cap = 0;
-  DevBuf<uint8_t> blob, verdict;
-  DevBuf<int32_t> best2, count;
-  DevBuf<float> X3;
-  DevBuf<ccm_new_point> out;
-  void release_device() {   // the blocks belong to the device they were allocated on
-    blob.release(); verdict.release(); best2.release(); count.release(); X3.release(); out.release();
-  }
-  ~Scratch() {
-    if (h_blob) cudaFreeHost(h_blob);
-    if (stream) cudaStreamDestroy(stream);
-  }
-};
-thread_local Scratch t_scr;
+// per-thread staging (Staging): LocalMapping calls once per keyframe
+thread_local Staging t_stage;
 
 // the View table (views[0] the current keyframe, then the neighbours) followed by every array the views point to
-size_t pack_views(Packer& pk, const ccm_newpts_view* cur, const ccm_newpts_neighbour* nb, int32_t n_nb, const std::vector<int32_t>& ent_node,
+void pack_views(Packer& pk, const ccm_newpts_view* cur, const ccm_newpts_neighbour* nb, int32_t n_nb, const std::vector<int32_t>& ent_node,
                   const std::vector<int32_t>& peer) {
   const int n_nodes1 = cur->v.fv->n_nodes;
   View* table = pk.host ? reinterpret_cast<View*>(pk.host + pk.at) : nullptr;
@@ -301,7 +284,6 @@ size_t pack_views(Packer& pk, const ccm_newpts_view* cur, const ccm_newpts_neigh
     v.aux = b < 0 ? pk.put(ent_node.data(), ent_node.size()) : pk.put(peer.data() + (size_t)b * n_nodes1, (size_t)n_nodes1);
     if (table) table[b + 1] = v;
   }
-  return pk.at;
 }
 
 }  // namespace
@@ -370,54 +352,39 @@ extern "C" int ccm_new_map_points(const ccm_newpts_view* cur, const ccm_newpts_n
     for (int b = 0; b < n_nb; b++) shared += shared_nodes(cur->v.fv, nb[b].view.v.fv, peer.data() + (size_t)b * n_nodes1);
     if (cells == 0 || ne1 == 0 || shared == 0 || !any_free(cur)) { fill_empty((int64_t)cells, n_out, best2, verdict); return; }
 
-    Scratch& s = t_scr;
-    if (s.device != current_device()) {
-      if (s.stream) { cudaStreamDestroy(s.stream); s.stream = nullptr; }
-      s.release_device();
-      s.device = current_device();
-    }
-    if (!s.stream) CCM_CUDA(cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking));
-
     std::vector<int32_t> ent_node(ne1);
     for (int a = 0; a < n_nodes1; a++)
       for (int k = cur->v.fv->node_ptr[a]; k < cur->v.fv->node_ptr[a + 1]; k++) ent_node[k] = a;
-    Packer measure;
-    const size_t bytes = pack_views(measure, cur, nb, n_nb, ent_node, peer);
-    if (s.h_cap < bytes) {
-      if (s.h_blob) cudaFreeHost(s.h_blob);
-      s.h_blob = nullptr; s.h_cap = 0;
-      CCM_CUDA(cudaMallocHost((void**)&s.h_blob, bytes + bytes / 4));
-      s.h_cap = bytes + bytes / 4;
-    }
-    if (s.blob.n < bytes) s.blob.alloc(bytes + bytes / 4);
-    if (s.best2.n < cells) { s.best2.alloc(cells + cells / 4); s.verdict.alloc(cells + cells / 4); s.X3.alloc(3 * (cells + cells / 4)); s.out.alloc(cells + cells / 4); }
-    if (!s.count.n) s.count.alloc(1);
-    Packer pk;
-    pk.host = s.h_blob; pk.dev = s.blob.p;
-    pack_views(pk, cur, nb, n_nb, ent_node, peer);
-    try {
-      CCM_CUDA(cudaMemcpyAsync(s.blob.p, s.h_blob, bytes, cudaMemcpyHostToDevice, s.stream));
-      CCM_CUDA(cudaMemsetAsync(s.best2.p, 0xff, cells * sizeof(int32_t), s.stream));
-      CCM_CUDA(cudaMemsetAsync(s.verdict.p, 0, cells, s.stream));
-      const View* d_views = reinterpret_cast<const View*>(s.blob.p);
-      k_np_candidates<<<dim3(div_up(ne1, CTA), n_nb), CTA, 0, s.stream>>>(d_views, s.best2.p);
+    // the output block holds only what the kernels write; the copies go from it to the caller's arrays
+    Packer lay;
+    const size_t at_best2 = lay.reserve(cells * sizeof(int32_t)), at_verdict = lay.reserve(cells), at_X3 = lay.reserve(3 * cells * sizeof(float)),
+                 at_out = lay.reserve(cells * sizeof(ccm_new_point)), at_count = lay.reserve(sizeof(int32_t));
+    Staging& s = t_stage;
+    s.run([&] {
+      s.upload([&](Packer& pk) { pack_views(pk, cur, nb, n_nb, ent_node, peer); }, lay.at, 0);
+      int32_t* d_best2 = reinterpret_cast<int32_t*>(s.out.p + at_best2);
+      uint8_t* d_verdict = s.out.p + at_verdict;
+      float* d_X3 = reinterpret_cast<float*>(s.out.p + at_X3);
+      ccm_new_point* d_out = reinterpret_cast<ccm_new_point*>(s.out.p + at_out);
+      int32_t* d_count = reinterpret_cast<int32_t*>(s.out.p + at_count);
+      CCM_CUDA(cudaMemsetAsync(d_best2, 0xff, cells * sizeof(int32_t), s.stream));
+      CCM_CUDA(cudaMemsetAsync(d_verdict, 0, cells, s.stream));
+      const View* d_views = reinterpret_cast<const View*>(s.in.p);
+      k_np_candidates<<<dim3(div_up(ne1, CTA), n_nb), CTA, 0, s.stream>>>(d_views, d_best2);
       CCM_LAUNCHED();
-      k_np_triangulate<<<dim3(div_up(n, CTA), n_nb), CTA, 0, s.stream>>>(d_views, s.best2.p, s.verdict.p, s.X3.p);
+      k_np_triangulate<<<dim3(div_up(n, CTA), n_nb), CTA, 0, s.stream>>>(d_views, d_best2, d_verdict, d_X3);
       CCM_LAUNCHED();
-      k_np_claim<<<1, CLAIM_CTA, 0, s.stream>>>(n, n_nb, s.best2.p, s.verdict.p, s.X3.p, s.out.p, s.count.p);
+      k_np_claim<<<1, CLAIM_CTA, 0, s.stream>>>(n, n_nb, d_best2, d_verdict, d_X3, d_out, d_count);
       CCM_LAUNCHED();
       int32_t count = 0;
-      s.count.download(&count, 1, s.stream);
+      CCM_CUDA(cudaMemcpyAsync(&count, d_count, sizeof(int32_t), cudaMemcpyDeviceToHost, s.stream));
       CCM_CUDA(cudaStreamSynchronize(s.stream));
       *n_out = count;
       if (capacity < count) too_small(f, capacity, count);
-      s.out.download(out, (size_t)count, s.stream);
-      if (best2) s.best2.download(best2, cells, s.stream);
-      if (verdict) s.verdict.download(verdict, cells, s.stream);
+      if (count) CCM_CUDA(cudaMemcpyAsync(out, d_out, (size_t)count * sizeof(ccm_new_point), cudaMemcpyDeviceToHost, s.stream));
+      if (best2) CCM_CUDA(cudaMemcpyAsync(best2, d_best2, cells * sizeof(int32_t), cudaMemcpyDeviceToHost, s.stream));
+      if (verdict) CCM_CUDA(cudaMemcpyAsync(verdict, d_verdict, cells, cudaMemcpyDeviceToHost, s.stream));
       CCM_CUDA(cudaStreamSynchronize(s.stream));
-    } catch (...) {
-      cudaStreamSynchronize(s.stream);   // nothing of this call may still read the pinned block or write the caller's arrays
-      throw;
-    }
+    });
   });
 }

@@ -6,7 +6,6 @@
 // over the observers that are not bad, and the scale-invariance distances from the reference keyframe.  Here: one thread per point,
 // the observer loop sequential in mObservations order (the f32 sum depends on it: no tree reduction), keyframe centres gathered from a
 // K x 12 B table that stays in L2.  Arithmetic in normal_depth_math.cuh; the host entry point runs the same body.
-#include <algorithm>
 #include <vector>
 
 #include "common.cuh"
@@ -88,9 +87,8 @@ extern "C" int ccm_normal_depth(int32_t n_kf, const float* kf_centre, const uint
     ensure_device();
     if (n_mp == 0) return;
     const int64_t E = obs_ptr[n_mp];
-    cudaStream_t s = nullptr;
-    CCM_CUDA(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
-    struct StreamGuard { cudaStream_t s; ~StreamGuard() { cudaStreamDestroy(s); } } guard{s};
+    const CallStream cs;
+    const cudaStream_t s = cs.s;
     DevBuf<float> d_centre, d_pos, d_sref, d_slast, d_normal, d_max, d_min;
     DevBuf<uint8_t> d_bad, d_status;
     DevBuf<int64_t> d_ptr;
@@ -102,9 +100,8 @@ extern "C" int ccm_normal_depth(int32_t n_kf, const float* kf_centre, const uint
     d_pos.upload(mp_pos, (size_t)n_mp * 3, s); d_ptr.upload(obs_ptr, (size_t)n_mp + 1, s); d_ref.upload(mp_ref, n_mp, s);
     d_sref.upload(mp_scale_ref, n_mp, s); d_slast.upload(mp_scale_last, n_mp, s);
     d_normal.alloc((size_t)n_mp * 3); d_max.alloc(n_mp); d_min.alloc(n_mp); d_status.alloc(n_mp); d_flag.alloc_zero(1, s);
-    const int grid = std::min(div_up(n_mp, 256), sm_count() * 8);
-    k_normal_depth<<<grid, 256, 0, s>>>(n_mp, n_kf, d_centre.p, d_bad.p, d_pos.p, d_ptr.p, d_obs.p, d_ref.p, d_sref.p, d_slast.p, d_normal.p,
-                                        d_max.p, d_min.p, d_status.p, d_flag.p);
+    k_normal_depth<<<grid_size(n_mp, 256), 256, 0, s>>>(n_mp, n_kf, d_centre.p, d_bad.p, d_pos.p, d_ptr.p, d_obs.p, d_ref.p, d_sref.p,
+                                                         d_slast.p, d_normal.p, d_max.p, d_min.p, d_status.p, d_flag.p);
     CCM_LAUNCHED();
     int flag = 0;
     d_normal.download(normal, (size_t)n_mp * 3, s);

@@ -333,17 +333,11 @@ struct PgoDevice {
 int pcg_max_of(const ccm_pgo_options* o) { return o->pcg_max_iter > 0 ? o->pcg_max_iter : 5000; }
 double pcg_tol_of(const ccm_pgo_options* o) { return o->pcg_tol > 0 ? o->pcg_tol : 1e-10; }
 
-struct StreamGuard {
-  cudaStream_t s;
-  StreamGuard() { CCM_CUDA(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking)); }
-  ~StreamGuard() { cudaStreamDestroy(s); }
-};
-
 void pgo_solve(const ccm_pgo_problem* p, const ccm_pgo_options* o, ccm_pgo_result* r) {
   const auto T0 = std::chrono::steady_clock::now();
   ensure_device();
   CCM_REQUIRE(p && o && r && p->K > 0 && p->E >= 0 && p->sim3 && p->fixed && r->sim3, "ccm_pgo_solve: bad argument");
-  StreamGuard sg;
+  const CallStream sg;
   const cudaStream_t s = sg.s;
   const int K = p->K;
   const PgoSetup S(p);
@@ -468,7 +462,7 @@ void sim3_debug_ops(int n, const double* u, const double* a, const double* b, in
   ensure_device();
   CCM_REQUIRE(n >= 0 && (n == 0 || (u && a && b && exp_u && log_a && mul_ab && inv_a && oplus_u_a)), "ccm_sim3_debug_ops: bad argument");
   if (n == 0) return;
-  StreamGuard sg;
+  const CallStream sg;
   DevBuf<double> du, da, db, o_exp, o_log, o_mul, o_inv, o_oplus;
   du.upload(u, (size_t)n * 7, sg.s); da.upload(a, (size_t)n * 8, sg.s); db.upload(b, (size_t)n * 8, sg.s);
   o_exp.alloc((size_t)n * 8); o_log.alloc((size_t)n * 7); o_mul.alloc((size_t)n * 8); o_inv.alloc((size_t)n * 8); o_oplus.alloc((size_t)n * 8);
@@ -484,7 +478,7 @@ void pgo_debug_edges(int n, const double* meas, const double* si, const double* 
   ensure_device();
   CCM_REQUIRE(n >= 0 && (n == 0 || (meas && si && sj && free_ij && err && Ji && Jj)), "ccm_pgo_debug_edges: bad argument");
   if (n == 0) return;
-  StreamGuard sg;
+  const CallStream sg;
   DevBuf<double> dm, di, dj, de, dJi, dJj;
   DevBuf<int> df;
   dm.upload(meas, (size_t)n * 8, sg.s); di.upload(si, (size_t)n * 8, sg.s); dj.upload(sj, (size_t)n * 8, sg.s);
@@ -509,7 +503,7 @@ void pgo_debug_system(const ccm_pgo_problem* p, const ccm_pgo_options* o, double
   if (paths) { paths[0] = S.pcg_block; paths[1] = S.c_agg; paths[2] = S.c_nc; paths[3] = 0; }
   if (!H || S.n == 0) return;
   CCM_REQUIRE(b && Minv && x && chi2 && pcg, "ccm_pgo_debug_system: bad argument");
-  StreamGuard sg;
+  const CallStream sg;
   PgoDevice D(S, p->sim3, sg.s);
   D.chi2_of(D.d_v.p, D.scal.p);
   D.linearize(D.d_v.p, p->fix_scale);

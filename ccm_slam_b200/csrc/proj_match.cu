@@ -302,9 +302,8 @@ void device_window_best(const ccm_feature_grid* g, const ccm_proj_queries* q, co
   const CellIndex cells(*g);
   std::vector<WinQuery> hq;
   fill_window_queries(cells, *q, hq);
-  cudaStream_t s = nullptr;
-  CCM_CUDA(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking));
-  struct StreamGuard { cudaStream_t s; ~StreamGuard() { cudaStreamDestroy(s); } } guard{s};
+  const CallStream cs;
+  const cudaStream_t s = cs.s;
   DevBuf<WinQuery> dQ; DevBuf<uint4> dqd, dkd; DevBuf<int> dptr, dfeat, doct, dbi, dbd; DevBuf<float2> dxy; DevBuf<float> dw;
   dQ.upload(hq.data(), hq.size(), s);
   dqd.upload(reinterpret_cast<const uint4*>(q->desc), (size_t)q->m * 2, s);

@@ -90,6 +90,36 @@ void dev_free(void* p) {
   cudaFreeAsync(p, g_alloc_stream[dev & 63]);
 }
 
+// ---- per-thread staging of the batched entry points -------------------------------------------------------------------------------
+Staging::~Staging() {
+  if (h_in) cudaFreeHost(h_in);
+  if (h_out) cudaFreeHost(h_out);
+  if (stream) cudaStreamDestroy(stream);
+}
+
+void Staging::use_current_device() {
+  if (device != current_device()) {
+    if (stream) { cudaStreamDestroy(stream); stream = nullptr; }
+    in.release(); out.release();
+    device = current_device();
+  }
+  if (!stream) CCM_CUDA(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking));
+}
+
+void Staging::reserve(size_t d_in, size_t d_out, size_t p_in, size_t p_out) {
+  auto pinned = [](uint8_t** p, size_t* cap, size_t bytes) {
+    if (*cap >= bytes) return;
+    if (*p) cudaFreeHost(*p);
+    *p = nullptr; *cap = 0;
+    CCM_CUDA(cudaMallocHost((void**)p, bytes + bytes / 4));
+    *cap = bytes + bytes / 4;
+  };
+  pinned(&h_in, &h_in_cap, p_in);
+  pinned(&h_out, &h_out_cap, p_out);
+  if (in.n < d_in) in.alloc(d_in + d_in / 4);
+  if (out.n < d_out) out.alloc(d_out + d_out / 4);
+}
+
 // ---- NCCL through dlopen: the single-GPU path has no link-time dependency on it ----
 typedef struct { char internal[128]; } ncclUniqueId_t;
 typedef int (*fn_ncclGetUniqueId)(ncclUniqueId_t*);

@@ -86,10 +86,10 @@ std::vector<HostKf> host_kfs(const ccm_fuse_kf* kfs, int32_t n_kf) {
   return v;
 }
 
-thread_local Scratch t_scr;
+thread_local Staging t_stage;
 
 // the Kf table followed by every array the kernel reads
-size_t pack(Packer& pk, const std::vector<HostKf>& kfs, const ccm_fuse_kf* src, const ccm_fuse_points* pts, Pts* dp) {
+void pack(Packer& pk, const std::vector<HostKf>& kfs, const ccm_fuse_kf* src, const ccm_fuse_points* pts, Pts* dp) {
   Kf* table = pk.host ? reinterpret_cast<Kf*>(pk.host + pk.at) : nullptr;
   pk.reserve(kfs.size() * sizeof(Kf));
   for (size_t r = 0; r < kfs.size(); r++) {
@@ -97,7 +97,6 @@ size_t pack(Packer& pk, const std::vector<HostKf>& kfs, const ccm_fuse_kf* src, 
     if (table) table[r] = k;
   }
   *dp = put_points(pk, pts);
-  return pk.at;
 }
 
 }  // namespace
@@ -128,27 +127,21 @@ extern "C" int ccm_search_and_fuse(const ccm_fuse_kf* kfs, int32_t n_kf, const c
       return;
     }
     const std::vector<HostKf> hk = host_kfs(kfs, n_kf);
-    Scratch& s = t_scr;
+    Staging& s = t_stage;
     Pts dp{};
-    Packer measure;
-    const size_t bytes = pack(measure, hk, kfs, pts, &dp);
-    s.prepare(bytes, (size_t)n_pairs);
-    Packer pk;
-    pk.host = s.h_blob; pk.dev = s.blob.p;
-    pack(pk, hk, kfs, pts, &dp);
     const int tiles = (n + 31) / 32;
     const long long n_warps = (long long)n_kf * tiles;
-    try {
-      CCM_CUDA(cudaMemcpyAsync(s.blob.p, s.h_blob, bytes, cudaMemcpyHostToDevice, s.stream));
-      k_sf_pairs<<<div_up(n_warps * 32, CTA), CTA, 0, s.stream>>>(reinterpret_cast<const Kf*>(s.blob.p), dp, n, tiles, (int)n_warps, s.out.p);
+    const size_t out_bytes = (size_t)n_pairs * sizeof(int32_t);
+    s.run([&] {
+      s.upload([&](Packer& pk) { pack(pk, hk, kfs, pts, &dp); }, out_bytes, out_bytes);
+      int32_t* d_out = reinterpret_cast<int32_t*>(s.out.p);
+      k_sf_pairs<<<div_up(n_warps * 32, CTA), CTA, 0, s.stream>>>(reinterpret_cast<const Kf*>(s.in.p), dp, n, tiles, (int)n_warps, d_out);
       CCM_LAUNCHED();
-      s.out.download(s.h_out, (size_t)n_pairs, s.stream);
+      CCM_CUDA(cudaMemcpyAsync(s.h_out, d_out, out_bytes, cudaMemcpyDeviceToHost, s.stream));
       CCM_CUDA(cudaStreamSynchronize(s.stream));
-    } catch (...) {
-      cudaStreamSynchronize(s.stream);   // nothing of this call may still read the pinned block
-      throw;
-    }
-    std::vector<int32_t> out(s.h_out, s.h_out + n_pairs);
+    });
+    const int32_t* h_out = reinterpret_cast<const int32_t*>(s.h_out);
+    std::vector<int32_t> out(h_out, h_out + n_pairs);
     int settled = 0;
     const HostPts hp(*pts);
     for (long long w = 0; w < n_pairs; w++) {

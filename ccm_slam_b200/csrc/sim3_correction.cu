@@ -171,7 +171,7 @@ std::vector<int32_t> validate(const std::string& f, const Args& a) {
 }
 
 // the block the kernels read, in one layout for measuring and for filling
-size_t pack(Packer& pk, const Args& a, const std::vector<int32_t>& kf_entry, In* in) {
+void pack(Packer& pk, const Args& a, const std::vector<int32_t>& kf_entry, In* in) {
   const size_t K = (size_t)a.n_kf, E = (size_t)a.n_e, P = (size_t)a.n_mp;
   in->kf_centre = pk.put(a.kf_centre, 3 * K);
   in->kf_bad = pk.put(a.kf_bad, K);
@@ -187,18 +187,19 @@ size_t pack(Packer& pk, const Args& a, const std::vector<int32_t>& kf_entry, In*
   in->mp_ref = pk.put(a.mp_ref, P);
   in->scale_ref = pk.put(a.scale_ref, P);
   in->scale_last = pk.put(a.scale_last, P);
-  return pk.at;
 }
 
-// offsets of each output in the output block
+// offsets of each output in the output block: the downloaded part, then Swi, which only the kernels use
 struct OutLayout {
-  size_t Tcw, centre, mp_entry, pos, normal, max_dist, min_dist, status, bytes;
+  size_t Tcw, centre, mp_entry, pos, normal, max_dist, min_dist, status, down, swi, bytes;
   explicit OutLayout(const Args& a) {
     Packer pk;
     const size_t E = (size_t)a.n_e, P = (size_t)a.n_mp;
     Tcw = pk.reserve(16 * E * sizeof(float)); centre = pk.reserve(3 * E * sizeof(float)); mp_entry = pk.reserve(P * sizeof(int32_t));
     pos = pk.reserve(3 * P * sizeof(float)); normal = pk.reserve(3 * P * sizeof(float)); max_dist = pk.reserve(P * sizeof(float));
     min_dist = pk.reserve(P * sizeof(float)); status = pk.reserve(P);
+    down = pk.at;
+    swi = pk.reserve(8 * E * sizeof(double));
     bytes = pk.at;
   }
   Out at(uint8_t* base) const {
@@ -218,33 +219,8 @@ void scatter(const Args& a, const Out& o) {
   }
 }
 
-// per-thread staging: one pinned block each way, device blocks grown on demand (a merge corrects a whole map, a loop a few dozen keyframes)
-struct Scratch {
-  cudaStream_t stream = nullptr;
-  int device = -1;
-  uint8_t* h_in = nullptr;
-  size_t h_in_cap = 0;
-  uint8_t* h_out = nullptr;
-  size_t h_out_cap = 0;
-  DevBuf<uint8_t> in, out;
-  DevBuf<double> swi;
-  ~Scratch() {
-    if (h_in) cudaFreeHost(h_in);
-    if (h_out) cudaFreeHost(h_out);
-    if (stream) cudaStreamDestroy(stream);
-  }
-};
-thread_local Scratch t_scr;
-
-void grow_pinned(uint8_t** p, size_t* cap, size_t bytes) {
-  if (*cap >= bytes) return;
-  if (*p) cudaFreeHost(*p);
-  *p = nullptr; *cap = 0;
-  CCM_CUDA(cudaMallocHost((void**)p, bytes + bytes / 4));
-  *cap = bytes + bytes / 4;
-}
-
-int grid_for(int64_t n) { return (int)std::max<int64_t>(1, std::min<int64_t>(div_up(n, CTA), (int64_t)sm_count() * 8)); }
+// per-thread staging (Staging): a merge corrects a whole map, a loop a few dozen keyframes
+thread_local Staging t_stage;
 
 }  // namespace
 
@@ -295,40 +271,22 @@ extern "C" int ccm_sim3_correction(int32_t n_kf, const float* kf_centre, const u
     ensure_device();
     if (n_e == 0 && n_mp == 0) return;
 
-    Scratch& s = t_scr;
-    if (s.device != current_device()) {   // the blocks belong to the device they were allocated on
-      if (s.stream) { cudaStreamDestroy(s.stream); s.stream = nullptr; }
-      s.in.release(); s.out.release(); s.swi.release();
-      s.device = current_device();
-    }
-    if (!s.stream) CCM_CUDA(cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking));
+    Staging& s = t_stage;
     In in{};
-    Packer measure;
-    const size_t bytes = pack(measure, a, kf_entry, &in);
     const OutLayout ol(a);
-    grow_pinned(&s.h_in, &s.h_in_cap, bytes);
-    grow_pinned(&s.h_out, &s.h_out_cap, ol.bytes);
-    if (s.in.n < bytes) s.in.alloc(bytes + bytes / 4);
-    if (s.out.n < ol.bytes) s.out.alloc(ol.bytes + ol.bytes / 4);
-    if (s.swi.n < 8 * (size_t)n_e) s.swi.alloc(8 * (size_t)n_e + 8);
-    Packer pk;
-    pk.host = s.h_in; pk.dev = s.in.p;
-    pack(pk, a, kf_entry, &in);
-    const Out out = ol.at(s.out.p);
-    try {
-      CCM_CUDA(cudaMemcpyAsync(s.in.p, s.h_in, bytes, cudaMemcpyHostToDevice, s.stream));
-      k_sc_entries<<<grid_for(std::max(n_e, n_mp)), CTA, 0, s.stream>>>(n_e, n_mp, in, out, s.swi.p);
+    s.run([&] {
+      s.upload([&](Packer& pk) { pack(pk, a, kf_entry, &in); }, ol.bytes, ol.down);
+      const Out out = ol.at(s.out.p);
+      double* swi = reinterpret_cast<double*>(s.out.p + ol.swi);
+      k_sc_entries<<<grid_size(std::max(n_e, n_mp), CTA), CTA, 0, s.stream>>>(n_e, n_mp, in, out, swi);
       CCM_LAUNCHED();
-      k_sc_claim<<<grid_for(a.n_slots()), CTA, 0, s.stream>>>(n_e, a.n_slots(), in, out);
+      k_sc_claim<<<grid_size(a.n_slots(), CTA), CTA, 0, s.stream>>>(n_e, a.n_slots(), in, out);
       CCM_LAUNCHED();
-      k_sc_points<<<grid_for(n_mp), CTA, 0, s.stream>>>(n_mp, in, out, s.swi.p);
+      k_sc_points<<<grid_size(n_mp, CTA), CTA, 0, s.stream>>>(n_mp, in, out, swi);
       CCM_LAUNCHED();
-      CCM_CUDA(cudaMemcpyAsync(s.h_out, s.out.p, ol.bytes, cudaMemcpyDeviceToHost, s.stream));
+      CCM_CUDA(cudaMemcpyAsync(s.h_out, s.out.p, ol.down, cudaMemcpyDeviceToHost, s.stream));
       CCM_CUDA(cudaStreamSynchronize(s.stream));
-    } catch (...) {
-      cudaStreamSynchronize(s.stream);   // nothing of this call may still read the pinned blocks
-      throw;
-    }
+    });
     scatter(a, ol.at(s.h_out));
   });
 }

@@ -577,12 +577,6 @@ __global__ void __launch_bounds__(ST) k_sim3_debug_system(const Sim3Prob* __rest
 template <typename T>
 void append(std::vector<T>& dst, const T* src, size_t n) { dst.insert(dst.end(), src, src + n); }
 
-struct StreamGuard {
-  cudaStream_t s = nullptr;
-  StreamGuard() { CCM_CUDA(cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking)); }
-  ~StreamGuard() { if (s) cudaStreamDestroy(s); }
-};
-
 // a batch of pose problems on the device: one PoseProb per problem, the correspondences of all problems back to back
 struct PoseBatch {
   std::vector<PoseProb> hp;
@@ -645,7 +639,7 @@ void pose_optimize(const ccm_pose_opt_problem* probs, int batch, ccm_pose_opt_re
   ensure_device();
   CCM_REQUIRE(batch >= 0 && (batch == 0 || (probs && res)), "ccm_pose_optimize: bad argument");
   if (batch == 0) return;
-  StreamGuard sg;
+  const CallStream sg;
   cudaStream_t s = sg.s;
   PoseBatch B(probs, batch, res, "ccm_pose_optimize: null array", s);
   const size_t tot = B.tot, t1 = std::max(tot, (size_t)1);
@@ -677,7 +671,7 @@ void sim3_optimize(const ccm_sim3_opt_problem* probs, int batch, ccm_sim3_opt_re
   ensure_device();
   CCM_REQUIRE(batch >= 0 && (batch == 0 || (probs && res)), "ccm_sim3_optimize: bad argument");
   if (batch == 0) return;
-  StreamGuard sg;
+  const CallStream sg;
   cudaStream_t s = sg.s;
   Sim3Batch B(probs, batch, res, "ccm_sim3_optimize: null array", s);
   const size_t tot = B.tot, t1 = std::max(tot, (size_t)1);
@@ -712,7 +706,7 @@ void pose_debug_system(const ccm_pose_opt_problem* probs, int batch, const uint8
   ensure_device();
   CCM_REQUIRE(batch >= 0 && (batch == 0 || (probs && delta_lambda && sys && solved)), "ccm_pose_debug_system: bad argument");
   if (batch == 0) return;
-  StreamGuard sg;
+  const CallStream sg;
   cudaStream_t s = sg.s;
   PoseBatch B(probs, batch, nullptr, "ccm_pose_debug_system: null array", s);
   const size_t tot = B.tot, t1 = std::max(tot, (size_t)1);
@@ -734,7 +728,7 @@ void sim3_debug_system(const ccm_sim3_opt_problem* probs, int batch, const uint8
   ensure_device();
   CCM_REQUIRE(batch >= 0 && (batch == 0 || (probs && delta_lambda && sys && solved)), "ccm_sim3_debug_system: bad argument");
   if (batch == 0) return;
-  StreamGuard sg;
+  const CallStream sg;
   cudaStream_t s = sg.s;
   Sim3Batch B(probs, batch, nullptr, "ccm_sim3_debug_system: null array", s);
   const size_t tot = B.tot, t1 = std::max(tot, (size_t)1);
