@@ -651,6 +651,40 @@ def sim3_correction(sc, host=False, out=None):
     return out
 
 
+KEYFRAME_CULLING_IN = (("kf_bad", np.uint8), ("cand_kf", np.int32), ("cand_not_erase", np.uint8), ("slot_ptr", np.int64),
+                       ("slot_mp", np.int32), ("slot_octave", np.int32), ("mp_bad", np.uint8), ("mp_nobs", np.int32), ("mp_ref", np.int32),
+                       ("obs_ptr", np.int64), ("obs_kf", np.int32), ("obs_octave", np.int32))
+
+
+def keyframe_culling_out(n_c):
+    """zeroed outputs of ccm_keyframe_culling for n_c candidates"""
+    return dict(cull=np.zeros(n_c, np.uint8), n_mps=np.zeros(n_c, np.int32), n_red=np.zeros(n_c, np.int32), n_settled=np.zeros(1, np.int32))
+
+
+def keyframe_culling_args(sc, out):
+    """(argument tuple of ccm_keyframe_culling, arrays it points into) for the flat arrays of a scene as
+    synth.make_keyframe_culling_scene builds it (th_obs and red_thres from the scene, 3 and 0.98 when absent)"""
+    a = {k: np.ascontiguousarray(sc[k], t) for k, t in KEYFRAME_CULLING_IN}
+    K, Cn, P = len(a["kf_bad"]), len(a["cand_kf"]), len(a["mp_bad"])
+    argv = (K, _p(a["kf_bad"]), Cn, _p(a["cand_kf"]), _p(a["cand_not_erase"]), _p(a["slot_ptr"]), _p(a["slot_mp"]), _p(a["slot_octave"]), P,
+            _p(a["mp_bad"]), _p(a["mp_nobs"]), _p(a["mp_ref"]), _p(a["obs_ptr"]), _p(a["obs_kf"]), _p(a["obs_octave"]), int(sc.get("th_obs", 3)),
+            C.c_double(float(sc.get("red_thres", 0.98))), _p(out["cull"]), _p(out["n_mps"]), _p(out["n_red"]), _p(out["n_settled"]))
+    return argv, a
+
+
+def keyframe_culling(sc, host=False, out=None):
+    """The redundancy test of LocalMapping::KeyFrameCullingV3 (cslam/src/Mapping.cpp:771-863) for every candidate, earlier culls
+    included, see include/ccm_b200.h.  sc: dict(kf_bad (K,) u8, cand_kf (C,) i32, cand_not_erase (C,) u8, slot_ptr (C+1,) i64, slot_mp,
+    slot_octave i32, mp_bad (P,) u8, mp_nobs (P,) i32, mp_ref (P,) i32, obs_ptr (P+1,) i64, obs_kf, obs_octave i32, th_obs, red_thres),
+    as synth.make_keyframe_culling_scene builds it.  Returns dict(cull (C,) u8, n_mps (C,) i32, n_red (C,) i32, n_settled int).
+    host=False: ccm_keyframe_culling on the GPU; host=True: ccm_keyframe_culling_host.  out: preallocated outputs (keyframe_culling_out)."""
+    out = keyframe_culling_out(len(sc["cand_kf"])) if out is None else out
+    argv, _keep = keyframe_culling_args(sc, out)
+    fn = lib().ccm_keyframe_culling_host if host else lib().ccm_keyframe_culling
+    _chk(fn(*argv))
+    return dict(cull=out["cull"], n_mps=out["n_mps"], n_red=out["n_red"], n_settled=int(out["n_settled"][0]))
+
+
 class NewPtsViewC(C.Structure):
     _fields_ = [("v", TriViewC), ("Tcw", C.c_float * 12), ("Ow", C.c_float * 3), ("level_sigma2", C.c_void_p),
                 ("scale_factors", C.c_void_p), ("nlevels", C.c_int32), ("scale_factor", C.c_float)]

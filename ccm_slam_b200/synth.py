@@ -792,3 +792,195 @@ def make_sim3_correction(p: BAProblem | None = None, kind="loop", seed=0, K=60, 
                 mp_skip=(mp_bad | tagged).astype(np.uint8), obs_ptr=obs_ptr, obs_kf=obs_kf.astype(np.int32), mp_ref=ref,
                 mp_scale_ref=sref, mp_scale_last=np.full(P, sf[-1], np.float32), kf_Tcw=Tcw, kf_rank=pk["kf_rank"], mp_bad=mp_bad,
                 mp_tagged=tagged, cur=cur)
+
+
+class _KcMap:
+    """A small mutable map for make_keyframe_culling_scene: keyframes with slots (point row or -1, keypoint octave), points with
+    observers (keyframe row, slot index) in mObservations order, nObs and mpRefKF."""
+
+    def __init__(self):
+        self.kf_bad, self.kf_not_erase, self.kf_id, self.slots = [], [], [], []
+        self.mp_bad, self.mp_nobs, self.mp_ref, self.obs = [], [], [], []
+
+    def kf(self, bad=0, not_erase=0, id=None):
+        self.kf_bad.append(bad); self.kf_not_erase.append(not_erase); self.slots.append([])
+        self.kf_id.append(len(self.kf_id) + 2 if id is None else id)
+        return len(self.kf_bad) - 1
+
+    def pt(self, observers, nobs=None, ref=0, bad=0):
+        """observers: (keyframe row, octave) each, in mObservations order; each gets a slot that holds the point.  ref: position in
+        observers of mpRefKF, or None for a null mpRefKF"""
+        p = len(self.mp_bad)
+        o = []
+        for k, octave in observers:
+            o.append((k, len(self.slots[k])))
+            self.slots[k].append((p, int(octave)))
+        self.obs.append(o)
+        self.mp_bad.append(bad)
+        self.mp_nobs.append(len(o) if nobs is None else nobs)
+        self.mp_ref.append(-1 if ref is None or not o else o[ref][0])
+        return p
+
+    def slot(self, k, p, octave):
+        """a slot of keyframe k that holds point p (or -1) without an observation of it"""
+        self.slots[k].append((p, int(octave)))
+
+    def redundant_points(self, k, n, observers, octave=0):
+        """n points in k's slots, each seen by k at `octave` and by every keyframe of `observers` at octave 0"""
+        return [self.pt([(k, octave)] + [(g, 0) for g in observers]) for _ in range(n)]
+
+    def arrays(self):
+        ids = np.asarray(self.kf_id, np.int64)
+        K, P = len(self.kf_bad), len(self.mp_bad)
+        obs = [sorted(o, key=lambda e: ids[e[0]]) if not self.mp_bad[p] else [] for p, o in enumerate(self.obs)]   # a bad point has none
+        sptr = np.zeros(K + 1, np.int64); sptr[1:] = np.cumsum([len(s) for s in self.slots])
+        smp = np.asarray([s[0] for row in self.slots for s in row], np.int32).reshape(-1)
+        soct = np.asarray([s[1] for row in self.slots for s in row], np.int32).reshape(-1)
+        optr = np.zeros(P + 1, np.int64); optr[1:] = np.cumsum([len(o) for o in obs])
+        okf = np.asarray([e[0] for o in obs for e in o], np.int32).reshape(-1)
+        oidx = np.asarray([e[1] for o in obs for e in o], np.int32).reshape(-1)
+        return dict(kf_bad=np.asarray(self.kf_bad, np.uint8), kf_not_erase=np.asarray(self.kf_not_erase, np.uint8), kf_id=ids.astype(np.int64),
+                    kf_slot_ptr=sptr, kf_slot_mp=smp, kf_slot_octave=soct, mp_bad=np.asarray(self.mp_bad, np.uint8).reshape(P),
+                    mp_nobs=np.asarray(self.mp_nobs, np.int32).reshape(P), mp_ref=np.asarray(self.mp_ref, np.int32).reshape(P),
+                    obs_ptr=optr, obs_kf=okf, obs_idx=oidx, obs_octave=soct[sptr[okf] + oidx] if len(okf) else np.zeros(0, np.int32))
+
+
+def keyframe_culling_candidates(sc):
+    """The flat candidate arrays of ccm_keyframe_culling for a map scene: the query's covisible keyframes, in order, without mId.first 0
+    or 1 and without the recently added ones (Mapping.cpp:799-805), each with its slots."""
+    recent = set(int(k) for k in sc["recent"])
+    cand = np.asarray([k for k in sc["covis"] if sc["kf_id"][k] not in (0, 1) and int(k) not in recent], np.int32)
+    sptr = sc["kf_slot_ptr"]
+    n = sptr[cand + 1] - sptr[cand]
+    ptr = np.zeros(len(cand) + 1, np.int64); ptr[1:] = np.cumsum(n)
+    idx = (np.repeat(sptr[cand] - ptr[:-1], n) + np.arange(ptr[-1])).astype(np.int64)
+    return dict(cand_kf=cand, cand_not_erase=sc["kf_not_erase"][cand], slot_ptr=ptr, slot_mp=sc["kf_slot_mp"][idx],
+                slot_octave=sc["kf_slot_octave"][idx])
+
+
+def make_keyframe_culling_scene(n_c=20, slots=1000, obs=(5, 20), seed=0, n_redundant=2, fresh_frac=0.1, null_frac=0.03, dup_frac=0.01,
+                                bad_mp_frac=0.02, bad_kf_frac=0.03, no_ref_frac=0.002, edges=True, red_thres=0.98, split=None):
+    """Inputs of ccm_keyframe_culling (the redundancy test of LocalMapping::KeyFrameCullingV3, include/ccm_b200.h) as a whole map:
+    keyframe rows with mvpMapPoints slots and keypoint octaves, points with observers, nObs and mpRefKF; the picked keyframe `query`,
+    its covisible list `covis` (rows 0 and 1 have mId.first 0 and 1) and mlpRecentAddedKFs `recent`; and the flat candidate arrays
+    (keyframe_culling_candidates).
+
+    Server-shaped part: n_c candidates of about `slots` slots each, points with obs[0]..obs[1] observers among the candidates and
+    n_c // 2 + 8 other keyframes, octaves drawn by the ORB level quotas; fresh_frac of each slot list holds points with two or three
+    observers (so an ordinary candidate stays below 0.98), null slots, a point at two slots, bad points and bad observers, points with
+    no mpRefKF.  n_redundant candidates see every point at octave 7 and are culled; their culls reach later candidates.
+
+    edges=True adds, each on its own keyframes: the 0.98 ties at nMPs 50 and 100; a point with Observations() == 3 and three other
+    observers; observers at octave level + 1 and level + 2; a point whose other counted observer is only the candidate itself; nMPs ==
+    0; a redundant candidate with mbNotErase and an already bad one; and three cascades (a cull drops a point to nObs <= 2 and turns a
+    later verdict to cull; a cull was mpRefKF of a point whose observers left are all bad, which changes an already bad candidate's
+    counts; a cull reaches points with no mpRefKF, one it does not observe).  split=(n, k): one candidate with n points of which k are
+    redundant, for the threshold test, and no other part."""
+    rng = np.random.default_rng(seed)
+    m = _KcMap()
+    order = []   # the candidates in covisibility order, built as a list of groups that keep their internal order
+    m.kf(id=0); m.kf(id=1)
+    query = m.kf()
+    recent = [m.kf(), m.kf()]
+    if split is not None:
+        n, k = split
+        c = m.kf()
+        g = [m.kf() for _ in range(4)]
+        m.redundant_points(c, k, g)
+        for _ in range(n - k):
+            m.pt([(c, 0), (g[0], 0), (g[1], 0)])
+        order.append([c])
+        n_c = 0
+    cands = [m.kf(bad=int(rng.random() < 0.05)) for _ in range(n_c)]
+    extras = [m.kf(bad=int(rng.random() < bad_kf_frac)) for _ in range(n_c // 2 + 8)]
+    if n_c:
+        designed = set(int(c) for c in rng.choice(cands, min(n_redundant, n_c), replace=False)) if n_redundant else set()
+        for c in designed:
+            m.kf_bad[c] = 0
+        pool = np.asarray(cands + extras + recent + [0, 1])
+        plain = np.asarray([k for k in pool if k not in designed])
+        q = OCTAVE_QUOTAS / OCTAVE_QUOTAS.sum()
+        avg = (obs[0] + obs[1]) / 2.0
+        P = int(slots * len(pool) * (1 - fresh_frac) / avg)
+        for _ in range(P):
+            d = min(int(rng.integers(obs[0], obs[1] + 1)), len(pool))
+            who = rng.choice(pool, d, replace=False)
+            octs = rng.choice(8, d, p=q)
+            octs[np.isin(who, list(designed))] = 7
+            m.pt(list(zip(who.tolist(), octs.tolist())), ref=int(rng.integers(d)) if rng.random() >= no_ref_frac else None,
+                 bad=int(rng.random() < bad_mp_frac))
+        for _ in range(int(slots * len(plain) * fresh_frac / 2.5)):
+            d = int(rng.integers(2, 4))
+            who = rng.choice(plain, d, replace=False)
+            m.pt(list(zip(who.tolist(), rng.choice(8, d, p=q).tolist())), ref=int(rng.integers(d)))
+        for c in cands:
+            held = [s[0] for s in m.slots[c] if s[0] >= 0]
+            for _ in range(int(len(held) * null_frac)):
+                m.slot(c, -1, int(rng.integers(8)))
+            for p in rng.choice(held, int(len(held) * dup_frac), replace=False) if held else []:
+                m.slot(c, int(p), 7 if c in designed else int(rng.integers(8)))
+        order += [[c] for c in cands]
+    if edges:
+        def good(n):
+            return [m.kf() for _ in range(n)]
+        for n in (50, 100):                                       # ties: nRedundant == 0.98 * nMPs exactly
+            c, g = m.kf(), good(4)
+            m.redundant_points(c, n - n // 50, g)
+            for _ in range(n // 50):
+                m.pt([(c, 0), (g[0], 0), (g[1], 0), (m.kf(bad=1), 0)])   # nObs 4, two counted others: the candidate itself is not one
+            order.append([c])
+        c, g = m.kf(), good(4)                                    # Observations() == 3 with three other observers: not redundant
+        m.redundant_points(c, 49, g)
+        m.slot(c, m.pt([(g[0], 0), (g[1], 0), (g[2], 0)]), 0)
+        order.append([c])
+        c, g = m.kf(), good(4)                                    # observers at level + 1 count (a cull) ...
+        for _ in range(50):
+            m.pt([(c, 2)] + [(x, 3) for x in g])
+        order.append([c])
+        c, g = m.kf(), good(4)                                    # ... at level + 2 they do not
+        for _ in range(50):
+            m.pt([(c, 2)] + [(x, 4) for x in g])
+        order.append([c])
+        c = m.kf()                                                # nMPs == 0: null slots and bad points only
+        for _ in range(3):
+            m.slot(c, -1, 0)
+        for _ in range(2):
+            m.pt([(c, 0)] + [(x, 0) for x in good(4)], bad=1)
+        order.append([c])
+        for flag in ("not_erase", "bad"):                         # redundant, reported, no effect; a later candidate shares its points
+            c = m.kf(bad=int(flag == "bad"), not_erase=int(flag == "not_erase"))
+            later, g = m.kf(), good(4)
+            for _ in range(50):
+                m.pt([(c, 7), (later, 0), (g[0], 0), (g[1], 0)])   # three counted others for later only while c is not bad
+            order.append([c, later])
+        a, b, g, g1 = m.kf(), m.kf(), good(4), m.kf()             # cascade 1: A's cull drops X to nObs 2, B then culls
+        m.redundant_points(a, 50, g, octave=7)
+        m.redundant_points(b, 49, g)
+        m.pt([(a, 7), (b, 0), (g1, 0)])
+        order.append([a, b])
+        a, c, g = m.kf(), m.kf(bad=1), good(4)                    # cascade 2: A was mpRefKF of Y, every observer left is bad
+        m.redundant_points(a, 50, g, octave=7)
+        m.redundant_points(c, 10, g, octave=7)
+        m.pt([(a, 0), (m.kf(bad=1), 0), (m.kf(bad=1), 0), (m.kf(bad=1), 0), (c, 7)], ref=0)
+        order.append([a, c])
+        a, b, g = m.kf(), m.kf(), good(4)                         # cascade 3: points with no mpRefKF, one not observed by A
+        m.redundant_points(a, 50, g, octave=7)
+        m.redundant_points(b, 49, g)
+        m.pt([(a, 7), (b, 0)] + [(x, 5) for x in g], ref=None)
+        w2 = m.pt([(b, 0)] + [(x, 5) for x in g], ref=None)
+        m.slot(a, w2, 7)
+        order.append([a, b])
+    # interleave the groups at random, keeping each group's order, then add the filtered rows
+    flat = []
+    groups = [list(g) for g in order]
+    while groups:
+        i = int(rng.integers(len(groups)))
+        flat.append(groups[i].pop(0))
+        if not groups[i]:
+            groups.pop(i)
+    for k in (0, 1) + tuple(recent):
+        flat.insert(int(rng.integers(len(flat) + 1)), k)
+    sc = m.arrays()
+    sc.update(query=query, covis=np.asarray(flat, np.int32), recent=np.asarray(recent, np.int32), th_obs=3, red_thres=float(red_thres))
+    sc.update(keyframe_culling_candidates(sc))
+    return sc

@@ -923,6 +923,49 @@ int ccm_sim3_correction_host(int32_t n_kf, const float* kf_centre, const uint8_t
                              float* entry_centre, int32_t* mp_entry, float* mp_pos_out, float* normal, float* max_dist, float* min_dist,
                              uint8_t* status);
 
+/* ---- keyframe culling --------------------------------------------------------------------------------------------------------
+ * The redundancy test of LocalMapping::KeyFrameCullingV3 (cslam/src/Mapping.cpp:771-863) for every covisible keyframe of the picked
+ * keyframe in one call, exactly (integer counts, one f64 comparison).  The random pick, the skips of mId.first 0 / 1 and of
+ * mlpRecentAddedKFs, and the SetBadFlag calls stay with the caller; the candidates arrive already filtered, in
+ * GetVectorCovisibleKeyFrames() order.
+ *
+ * For candidate c (row cand_kf[c]): nMPs counts the slots whose point is not null and not bad (a point at two slots counts twice);
+ * nRedundant counts those whose point has nObs > th_obs and at least th_obs observers other than the candidate that are not bad and
+ * whose keypoint octave is <= the slot's octave + 1.  cull[c] = nRedundant > red_thres * nMPs, in f64, strictly.
+ *
+ * Why one pass plus a host settle is exact: a cull that takes effect (the candidate is not bad and cand_not_erase is 0) changes
+ * what later candidates read — the culled keyframe turns bad, and MapPoint::EraseObservation on each of its slots' points decrements
+ * nObs, moves mpRefKF off it and can turn the point bad (nObs <= 2 after the erase, no observer left that is not bad, or mpRefKF
+ * already null).  Those are the only changes, and they reach only points in the culled keyframe's slots or points that list it as an
+ * observer.  So every candidate is counted over the state at the start of the member; the host then walks the candidates in order,
+ * applies each effective cull and counts again a later candidate with a slot whose point an earlier cull touched.  *n_settled (may
+ * be NULL) counts those candidates.  Both steps share ccm_slam_b200/csrc/keyframe_culling_math.cuh.
+ *
+ *   kf_bad [n_kf]          isBad() of each keyframe row at the start of the member
+ *   cand_kf [n_c]          the candidate rows (each row at most once);  cand_not_erase [n_c]: mbNotErase (SetBadFlag only sets
+ *                          mbToBeErased then: the verdict is reported and has no effect)
+ *   slot_ptr [n_c+1], slot_mp, slot_octave [slot_ptr[n_c]]   candidate c's GetMapPointMatches() in index order as point rows (-1 null)
+ *                          and pKF->mvKeysUn[i].octave of each slot
+ *   mp_bad, mp_nobs, mp_ref [n_mp]   isBad(), the nObs counter as given (Observations()), the row of mpRefKF (-1 null)
+ *   obs_ptr [n_mp+1], obs_kf, obs_octave [obs_ptr[n_mp]]     each point's observers in mObservations order (each keyframe at most once)
+ *                          and pKFi->mvKeysUn[idx].octave of each observation
+ *   th_obs                 thObs (3 in the reference);  red_thres: mfRedundancyThres (Mapping.RedThres)
+ * Out: cull [n_c] (1: the member calls SetBadFlag and counts a cull), n_mps / n_red [n_c] (the two counts the decision compared, after
+ * earlier culls).  A row out of range, a candidate listed twice or a null array fails with CCM_ERR_INVALID and a message naming the
+ * candidate or point; nothing is written then.  No candidates: no launch.
+ * ccm_keyframe_culling: one pinned upload, one launch (one CTA per candidate), one download; integer reductions only, identical bytes
+ * every call.  ccm_keyframe_culling_host: the same contract without a device; the two agree bit for bit. */
+int ccm_keyframe_culling(int32_t n_kf, const uint8_t* kf_bad, int32_t n_c, const int32_t* cand_kf, const uint8_t* cand_not_erase,
+                         const int64_t* slot_ptr, const int32_t* slot_mp, const int32_t* slot_octave, int32_t n_mp, const uint8_t* mp_bad,
+                         const int32_t* mp_nobs, const int32_t* mp_ref, const int64_t* obs_ptr, const int32_t* obs_kf,
+                         const int32_t* obs_octave, int32_t th_obs, double red_thres, uint8_t* cull, int32_t* n_mps, int32_t* n_red,
+                         int32_t* n_settled);
+int ccm_keyframe_culling_host(int32_t n_kf, const uint8_t* kf_bad, int32_t n_c, const int32_t* cand_kf, const uint8_t* cand_not_erase,
+                              const int64_t* slot_ptr, const int32_t* slot_mp, const int32_t* slot_octave, int32_t n_mp,
+                              const uint8_t* mp_bad, const int32_t* mp_nobs, const int32_t* mp_ref, const int64_t* obs_ptr,
+                              const int32_t* obs_kf, const int32_t* obs_octave, int32_t th_obs, double red_thres, uint8_t* cull,
+                              int32_t* n_mps, int32_t* n_red, int32_t* n_settled);
+
 #ifdef __cplusplus
 }
 #endif
