@@ -1,6 +1,6 @@
 // ccm_covis_double.cpp — TEST INFRASTRUCTURE: a CPU double of the device entry point ccm_covisibility (include/ccm_b200.h), so that
 // shim/KeyFrameConnections_shim.cpp can be linked and run without a GPU.  The values come from the oracle (covis_oracle.cpp);
-// ccm_covisibility_host stays the product library's own.  Linked with -Bsymbolic in front of libccm_b200.so (oracle/covis.mk).
+// ccm_covisibility_host stays the product library's own.  Linked with -Bsymbolic in front of libccm_b200.so (oracle/Makefile).
 #include <cstdint>
 
 #include "ccm_b200.h"

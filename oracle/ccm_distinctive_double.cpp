@@ -2,7 +2,7 @@
 // ccm_kfstore_distinctive_descriptors (include/ccm_b200.h), so that shim/MapPointDescriptor_shim.cpp can be linked and run without a
 // GPU.  The values come from the oracle (distinctive_oracle.cpp); ccm_distinctive_descriptors_host stays the product library's own.
 // The store double holds descriptors put through dd_double_store_put under their uid; any non-null ccm_kf_store* names it.
-// Linked with -Bsymbolic in front of libccm_b200.so (oracle/distinctive.mk).
+// Linked with -Bsymbolic in front of libccm_b200.so (oracle/Makefile).
 #include <cstddef>
 #include <cstdint>
 #include <map>

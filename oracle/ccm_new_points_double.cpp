@@ -1,6 +1,6 @@
 // ccm_new_points_double.cpp — TEST INFRASTRUCTURE: a CPU double of the device entry point ccm_new_map_points (include/ccm_b200.h), so
 // that shim/NewMapPoints_shim.cpp can be linked and run without a GPU.  The values come from the sequential oracle
-// (new_points_oracle.cpp).  Linked with -Bsymbolic in front of libccm_b200.so (oracle/new_points.mk).
+// (new_points_oracle.cpp).  Linked with -Bsymbolic in front of libccm_b200.so (oracle/Makefile).
 #include <cstdint>
 
 #include "ccm_b200.h"

@@ -1,6 +1,6 @@
 // ccm_normal_depth_double.cpp — TEST INFRASTRUCTURE: a CPU double of the device entry point ccm_normal_depth (include/ccm_b200.h),
 // so that shim/MapPoint_shim.cpp can be linked and run without a GPU.  The values come from the oracle (normal_depth_oracle.cpp);
-// ccm_normal_depth_host stays the product library's own.  Linked with -Bsymbolic in front of libccm_b200.so (oracle/normal_depth.mk).
+// ccm_normal_depth_host stays the product library's own.  Linked with -Bsymbolic in front of libccm_b200.so (oracle/Makefile).
 #include <cstdint>
 
 #include "ccm_b200.h"

@@ -1,5 +1,5 @@
 // ccm_sim3_correction_double.cpp — TEST INFRASTRUCTURE: a CPU double of the device entry point ccm_sim3_correction (include/ccm_b200.h),
-// so that shim/Sim3Correction_shim.cpp runs on a machine without a GPU: the flat oracle (libsim3_correction_oracle.so) answers the call.
+// so that shim/Sim3Correction_shim.cpp runs on a machine without a GPU: the flat oracle (orc_sim3_correction of liboracle.so) answers the call.
 // Linked with -Bsymbolic into the shim test library ahead of libccm_b200.so; the GPU suite links the real entry point instead.
 #include <cstdint>
 

@@ -8,7 +8,7 @@
 // The marker members the queries use as scratch (mLoopQuery, mMatchQuery, mnLoopWords, mLoopScore, mRelocQuery, mnRelocWords,
 // mRelocScore) are kept per keyframe and read back by the tests; they start as the reference's constructor leaves them
 // (S/KeyFrame.cpp:39,56: the query ids = defpair, the counts 0) and the two scores, which the reference leaves uninitialised, at 0.
-// Built as oracle/libkfdb_oracle.so by oracle/kfdb.mk.
+// Built into oracle/liboracle.so by oracle/Makefile.
 #include <cfloat>
 #include <cmath>
 #include <cstdint>

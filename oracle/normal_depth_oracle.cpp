@@ -5,7 +5,7 @@
 //   cv::norm(normali)                    sqrt of the f64 sum, in index order, of the f64 squares of the f32 components
 //   normal + normali / norm              cv::scaleAdd(normali, 1.0 / norm, normal): fmaf with the scale rounded to float
 //   normal / n                           Mat::convertTo(CV_32F, 1.0 / n, 0): x * (float)(1.0 / n) + 0.f
-// Compiled by oracle/normal_depth.mk with -ffp-contract=off.
+// Compiled by oracle/Makefile with -ffp-contract=off.
 #include <cmath>
 #include <cstdint>
 

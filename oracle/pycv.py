@@ -1,6 +1,6 @@
-"""ctypes binding of the covisibility checker (oracle/covis.mk).  TEST INFRASTRUCTURE, NOT PRODUCT.
+"""ctypes binding of the covisibility checker (oracle/Makefile).  TEST INFRASTRUCTURE, NOT PRODUCT.
 
-  oracle(sc, th)          oracle/libcovis_oracle.so: our restatement of UpdateConnections' counter and orders over the flat arrays
+  oracle(sc, th)          oracle/liboracle.so (covis_oracle.cpp): our restatement of UpdateConnections' counter and orders over the flat arrays
   StandIn(sc, gpu=False)  a scene of stand-in KeyFrame / MapPoint objects (oracle/ref_stub_cv), keyframe row k at address rank
                           sc["kf_rank"][k], with .literal_flat() (the reference body's counter and ordered list per batch keyframe),
                           .merge(mode), .merge_stale(kind, row), .load_map(split) and .members(); over the CPU double of the device
@@ -10,30 +10,14 @@ The flat results are dicts shaped as api.covisibility's.
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_LIBS = {}
-
-
-def build() -> None:
-    subprocess.check_call(["make", "-C", _HERE, "-s", "-f", "covis.mk", "ref"])
+from oracle import pyoracle
 
 
 def _p(a):
     return a.ctypes.data_as(C.c_void_p)
-
-
-def _lib(name):
-    if name not in _LIBS:
-        so = os.path.join(_HERE, name)
-        if not os.path.exists(so):
-            build()
-        _LIBS[name] = C.CDLL(so)
-    return _LIBS[name]
 
 
 def _flat(B, cap):
@@ -55,7 +39,7 @@ def oracle(sc, th=15, batch=None):
     a = [np.ascontiguousarray(sc[k], t) for k, t in (("kf_id", np.uint64), ("kf_rank", np.uint32), ("mp_bad", np.uint8),
                                                      ("obs_ptr", np.int64), ("obs_kf", np.int32))]
     total = np.zeros(1, np.int64)
-    L = _lib("libcovis_oracle.so")
+    L = pyoracle.lib()
     L.orc_covisibility(len(a[0]), _p(a[0]), _p(a[1]), len(b), _p(b), _p(mptr), _p(mp), len(a[2]), _p(a[2]), _p(a[3]), _p(a[4]), int(th),
                        C.c_int64(0), None, None, None, None, None, None, None, _p(total))
     o = _flat(len(b), int(total[0]))
@@ -71,7 +55,7 @@ class StandIn:
     def __init__(self, sc, gpu=False, first_connection=None, fill_mvp=True):
         """first_connection: (K,) u8 mbFirstConnection of each row (None: all true); fill_mvp=False leaves mvpMapPoints empty (for
         load_map)"""
-        self.L = _lib(os.path.join("_ref", "libcovis_shim_gpu.so" if gpu else "libcovis_shim.so"))
+        self.L = pyoracle.ref_lib("libcovis_shim_gpu.so" if gpu else "libcovis_shim.so")
         self.L.cv_scene_create.restype = C.c_void_p
         self.L.cv_scene_destroy.argtypes = [C.c_void_p]
         for f in ("cv_merge", "cv_load_map"):

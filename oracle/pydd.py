@@ -1,6 +1,6 @@
-"""ctypes binding of the map-point descriptor checker (oracle/distinctive.mk).  TEST INFRASTRUCTURE, NOT PRODUCT.
+"""ctypes binding of the map-point descriptor checker (oracle/Makefile).  TEST INFRASTRUCTURE, NOT PRODUCT.
 
-  oracle(sc)             oracle/libdistinctive_oracle.so: our restatement of MapPoint::ComputeDistinctiveDescriptors over the flat arrays
+  oracle(sc)             oracle/liboracle.so (distinctive_oracle.cpp): our restatement of MapPoint::ComputeDistinctiveDescriptors over the flat arrays
   StandIn(sc, gpu=False) a scene of stand-in MapPoint / KeyFrame objects (oracle/ref_stub_dd) with .literal() (the reference body restated
                          on them), .shim(prepare) (shim/MapPointDescriptor_shim.cpp's member, with or without the batched preparation),
                          .stale(kind, kf), .search_in_neighbors(pts) and .establish(kf, mp_of_idx, split); over the CPU doubles of the
@@ -10,30 +10,14 @@ The oracle and .literal() return dict(best, best_median, desc); the shim calls r
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_LIBS = {}
-
-
-def build() -> None:
-    subprocess.check_call(["make", "-C", _HERE, "-s", "-f", "distinctive.mk", "ref"])
+from oracle import pyoracle
 
 
 def _p(a):
     return a.ctypes.data_as(C.c_void_p)
-
-
-def _lib(name):
-    if name not in _LIBS:
-        so = os.path.join(_HERE, name)
-        if not os.path.exists(so):
-            build()
-        _LIBS[name] = C.CDLL(so)
-    return _LIBS[name]
 
 
 def _choice(P):
@@ -43,7 +27,7 @@ def _choice(P):
 def oracle(sc):
     K = len(sc["kf_bad"]); P = len(sc["obs_ptr"]) - 1; o = _choice(P)
     a = [np.ascontiguousarray(sc[k], t) for k, t in (("kf_bad", np.uint8), ("obs_ptr", np.int64), ("obs_kf", np.int32), ("obs_desc", np.uint8))]
-    rc = _lib("libdistinctive_oracle.so").orc_distinctive_descriptors(K, _p(a[0]), P, _p(a[1]), _p(a[2]), _p(a[3]), _p(o["best"]),
+    rc = pyoracle.lib().orc_distinctive_descriptors(K, _p(a[0]), P, _p(a[1]), _p(a[2]), _p(a[3]), _p(o["best"]),
                                                                       _p(o["best_median"]), _p(o["desc"]))
     if rc != 0:
         raise ValueError("orc_distinctive_descriptors: bad input")
@@ -52,7 +36,7 @@ def oracle(sc):
 
 class StandIn:
     def __init__(self, sc, gpu=False):
-        self.L = _lib(os.path.join("_ref", "libdistinctive_shim_gpu.so" if gpu else "libdistinctive_shim.so"))
+        self.L = pyoracle.ref_lib("libdistinctive_shim_gpu.so" if gpu else "libdistinctive_shim.so")
         self.gpu = gpu
         self.L.dd_scene_create.restype = C.c_void_p
         self.L.dd_scene_destroy.argtypes = [C.c_void_p]

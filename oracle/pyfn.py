@@ -1,33 +1,16 @@
-"""ctypes binding of the neighbour-fusion checker (oracle/fuse_neighbours.mk).  TEST INFRASTRUCTURE, NOT PRODUCT.
+"""ctypes binding of the neighbour-fusion checker (oracle/Makefile).  TEST INFRASTRUCTURE, NOT PRODUCT.
 
-  oracle(sc)   oracle/libfuse_neighbours_oracle.so: every pair LocalMapping::SearchInNeighbors searches, Fuse's prelude with the host's
+  oracle(sc)   oracle/liboracle.so (fuse_neighbours_oracle.cpp): every pair LocalMapping::SearchInNeighbors searches, Fuse's prelude with the host's
                logf and the reference-pinned window search, over a scene as synth_match.make_fuse_scene builds it -> (fwd, bwd), shaped
                as api.fuse_neighbours' first two results
 """
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_LIB = None
-
-
-def build() -> None:
-    subprocess.check_call(["make", "-C", _HERE, "-s", "-f", "fuse_neighbours.mk", "ref"])
-
-
-def lib():
-    global _LIB
-    if _LIB is None:
-        so = os.path.join(_HERE, "libfuse_neighbours_oracle.so")
-        if not os.path.exists(so):
-            build()
-        _LIB = C.CDLL(so)
-    return _LIB
+from oracle import pyoracle
 
 
 def oracle(sc):
@@ -36,8 +19,8 @@ def oracle(sc):
     cur, tg, T, pts, cp, cand = api.fuse_structs(sc, keep)
     fwd = np.full((T, len(cp)), -3, np.int32)
     bwd = np.full(len(cand), -3, np.int32)
-    lib().orc_fuse_neighbours(C.byref(cur), tg, T, C.byref(pts), cp.ctypes.data_as(C.c_void_p), cand.ctypes.data_as(C.c_void_p), len(cand),
-                              fwd.ctypes.data_as(C.c_void_p), bwd.ctypes.data_as(C.c_void_p))
+    pyoracle.lib().orc_fuse_neighbours(C.byref(cur), tg, T, C.byref(pts), cp.ctypes.data_as(C.c_void_p), cand.ctypes.data_as(C.c_void_p), len(cand),
+                                       fwd.ctypes.data_as(C.c_void_p), bwd.ctypes.data_as(C.c_void_p))
     return fwd, bwd
 
 
@@ -49,10 +32,7 @@ class StandIn:
 
     def __init__(self, sc, gpu=False):
         from ccm_slam_b200 import api
-        so = os.path.join(_HERE, "_ref", "libfuse_neighbours_shim_gpu.so" if gpu else "libfuse_neighbours_shim.so")
-        if not os.path.exists(so):
-            build()
-        self.L = C.CDLL(so)
+        self.L = pyoracle.ref_lib("libfuse_neighbours_shim_gpu.so" if gpu else "libfuse_neighbours_shim.so")
         self.L.fn_scene_create.restype = C.c_void_p
         self.L.fn_scene_destroy.argtypes = [C.c_void_p]
         self.L.fn_run.argtypes = [C.c_void_p, C.c_int]

@@ -1,6 +1,6 @@
-"""ctypes binding of the keyframe-culling checker (oracle/keyframe_culling.mk).  TEST INFRASTRUCTURE, NOT PRODUCT.
+"""ctypes binding of the keyframe-culling checker (oracle/Makefile).  TEST INFRASTRUCTURE, NOT PRODUCT.
 
-  oracle(sc, slip=0)   oracle/libkeyframe_culling_oracle.so: LocalMapping::KeyFrameCullingV3 walked literally over live state, on the
+  oracle(sc, slip=0)   oracle/liboracle.so (keyframe_culling_oracle.cpp): LocalMapping::KeyFrameCullingV3 walked literally over live state, on the
                        flat arrays of ccm_keyframe_culling -> dict(cull, n_mps, n_red) as api.keyframe_culling returns them (without
                        n_settled).  slip selects a deliberately wrong reading: 1 `>=`, 2 the f32 threshold, 3 no cascade, 4 the
                        candidate's own observation counted, 5 `<` on the octave.
@@ -8,35 +8,19 @@
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_LIB = None
+from oracle import pyoracle
+
 SLIPS = {"ge": 1, "f32": 2, "no_cascade": 3, "own": 4, "octave_lt": 5}
-
-
-def build() -> None:
-    subprocess.check_call(["make", "-C", _HERE, "-s", "-f", "keyframe_culling.mk", "ref"])
-
-
-def lib():
-    global _LIB
-    if _LIB is None:
-        so = os.path.join(_HERE, "libkeyframe_culling_oracle.so")
-        if not os.path.exists(so):
-            build()
-        _LIB = C.CDLL(so)
-    return _LIB
 
 
 def oracle(sc, slip=0):
     from ccm_slam_b200 import api
     out = api.keyframe_culling_out(len(sc["cand_kf"]))
     argv, _keep = api.keyframe_culling_args(sc, out)
-    if lib().orc_keyframe_culling(*argv[:-1], int(slip)) != 0:
+    if pyoracle.lib().orc_keyframe_culling(*argv[:-1], int(slip)) != 0:
         raise ValueError("orc_keyframe_culling: bad input")
     return dict(cull=out["cull"], n_mps=out["n_mps"], n_red=out["n_red"])
 
@@ -49,10 +33,7 @@ class StandIn:
     shim/KeyFrameCulling_shim.cpp; over the host entry point standing in for the device, or the real library with gpu=True."""
 
     def __init__(self, sc, gpu=False, picks=None, checked=()):
-        so = os.path.join(_HERE, "_ref", "libkeyframe_culling_shim_gpu.so" if gpu else "libkeyframe_culling_shim.so")
-        if not os.path.exists(so):
-            build()
-        self.L = C.CDLL(so)
+        self.L = pyoracle.ref_lib("libkeyframe_culling_shim_gpu.so" if gpu else "libkeyframe_culling_shim.so")
         self.L.kc_scene_create.restype = C.c_void_p
         self.L.kc_scene_destroy.argtypes = [C.c_void_p]
         self.L.kc_run.argtypes = [C.c_void_p, C.c_int]

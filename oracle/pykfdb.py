@@ -1,6 +1,6 @@
-"""ctypes binding of the keyframe-database checker (oracle/kfdb.mk).  TEST INFRASTRUCTURE, NOT PRODUCT.
+"""ctypes binding of the keyframe-database checker (oracle/Makefile).  TEST INFRASTRUCTURE, NOT PRODUCT.
 
-  Oracle(n_words, scoring)     oracle/libkfdb_oracle.so: our restatement of S/Database.cpp's queries and DBoW2's six scores
+  Oracle(n_words, scoring)     oracle/liboracle.so (kfdb_oracle.cpp): our restatement of S/Database.cpp's queries and DBoW2's six scores
   Reference(n_words, scoring)  oracle/_ref/libkfdb_ref.so: the reference's own Database.cpp / ScoringObject.cpp compiled in place
                                against stand-in KeyFrame / Map / Frame records (None where neither the reference tree nor a
                                prebuilt library is present)
@@ -12,48 +12,24 @@ return the vector<kfptr> as uids; marker members can be read back after every ca
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_REF_TREE = "/root/reference/cslam/src/Database.cpp"
+from oracle import pyoracle
+
 NONE = np.uint64(0xFFFFFFFFFFFFFFFF)     # defpair
 _LIBS = {}
-
-
-def build(force: bool = False) -> str:
-    so = os.path.join(_HERE, "libkfdb_oracle.so")
-    src = os.path.join(_HERE, "kfdb_oracle.cpp")
-    if force or not os.path.exists(so) or os.path.getmtime(src) > os.path.getmtime(so):
-        subprocess.check_call(["make", "-C", _HERE, "-s", "-f", "kfdb.mk", "libkfdb_oracle.so"])
-    return so
-
-
-def build_ref() -> str | None:
-    so = os.path.join(_HERE, "_ref", "libkfdb_ref.so")
-    if os.path.exists(_REF_TREE):
-        subprocess.check_call(["make", "-C", _HERE, "-s", "-f", "kfdb.mk", "ref"])
-    return so if os.path.exists(so) else None
-
-
-_SHIM_SO = {"shim": "libkfdb_shim.so", "shim_gpu": "libkfdb_shim_gpu.so"}
+_REF_SO = {"ref": "libkfdb_ref.so", "shim": "libkfdb_shim.so", "shim_gpu": "libkfdb_shim_gpu.so"}
 
 
 def _load(kind):
     """kind: "orc" (the oracle), "ref" (the reference's Database.cpp), "shim" / "shim_gpu" (shim/Database_shim.cpp over the CPU double /
     the real device library); the last three share ref_kfdb_wrap.cpp's C interface"""
     if kind not in _LIBS:
-        so = build() if kind == "orc" else build_ref()
-        if so is None:
+        L = pyoracle.lib() if kind == "orc" else pyoracle.ref_lib(_REF_SO[kind])
+        if L is None:
             return None
-        if kind in _SHIM_SO:
-            so = os.path.join(_HERE, "_ref", _SHIM_SO[kind])
-            if not os.path.exists(so):
-                return None
         prefix = "orc" if kind == "orc" else "ref"
-        L = C.CDLL(so)
         f = lambda name: getattr(L, f"{prefix}_{name}")
         f("kfdb_create").restype = C.c_void_p
         f("kfdb_create").argtypes = [C.c_int32, C.c_int32]

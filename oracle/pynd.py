@@ -1,6 +1,6 @@
-"""ctypes binding of the map-point normal checker (oracle/normal_depth.mk).  TEST INFRASTRUCTURE, NOT PRODUCT.
+"""ctypes binding of the map-point normal checker (oracle/Makefile).  TEST INFRASTRUCTURE, NOT PRODUCT.
 
-  oracle(sc)             oracle/libnormal_depth_oracle.so: our restatement of MapPoint::UpdateNormalAndDepth over the flat arrays
+  oracle(sc)             oracle/liboracle.so (normal_depth_oracle.cpp): our restatement of MapPoint::UpdateNormalAndDepth over the flat arrays
   StandIn(sc, gpu=False) a scene of stand-in MapPoint / KeyFrame objects (oracle/ref_stub_mp) with .literal() (the reference body restated
                          on them), .shim(prepare) (shim/MapPoint_shim.cpp's member, with or without the batched preparation) and
                          .stale(kind, kf, shift); over the CPU double of ccm_normal_depth, or the real library with gpu=True
@@ -9,30 +9,14 @@ Every call returns dict(normal, max_dist, min_dist, status).
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_LIBS = {}
-
-
-def build() -> None:
-    subprocess.check_call(["make", "-C", _HERE, "-s", "-f", "normal_depth.mk", "ref"])
+from oracle import pyoracle
 
 
 def _p(a):
     return a.ctypes.data_as(C.c_void_p)
-
-
-def _lib(name):
-    if name not in _LIBS:
-        so = os.path.join(_HERE, name)
-        if not os.path.exists(so):
-            build()
-        _LIBS[name] = C.CDLL(so)
-    return _LIBS[name]
 
 
 def _out(P):
@@ -48,7 +32,7 @@ def oracle(sc):
     K = len(sc["kf_bad"]); P = len(sc["mp_ref"]); o = _out(P)
     a = [np.ascontiguousarray(sc[k], t) for k, t in (("kf_centre", np.float32), ("kf_bad", np.uint8), ("mp_pos", np.float32), ("obs_ptr", np.int64),
                                                      ("obs_kf", np.int32), ("mp_ref", np.int32), ("mp_scale_ref", np.float32), ("mp_scale_last", np.float32))]
-    rc = _lib("libnormal_depth_oracle.so").orc_normal_depth(K, _p(a[0]), _p(a[1]), P, _p(a[2]), _p(a[3]), _p(a[4]), _p(a[5]), _p(a[6]), _p(a[7]), *_args(o))
+    rc = pyoracle.lib().orc_normal_depth(K, _p(a[0]), _p(a[1]), P, _p(a[2]), _p(a[3]), _p(a[4]), _p(a[5]), _p(a[6]), _p(a[7]), *_args(o))
     if rc != 0:
         raise ValueError("orc_normal_depth: bad input")
     return o
@@ -56,7 +40,7 @@ def oracle(sc):
 
 class StandIn:
     def __init__(self, sc, gpu=False):
-        self.L = _lib(os.path.join("_ref", "libnormal_depth_shim_gpu.so" if gpu else "libnormal_depth_shim.so"))
+        self.L = pyoracle.ref_lib("libnormal_depth_shim_gpu.so" if gpu else "libnormal_depth_shim.so")
         self.L.nd_scene_create.restype = C.c_void_p
         self.L.nd_scene_destroy.argtypes = [C.c_void_p]
         self.L.nd_shim_stale.argtypes = [C.c_void_p, C.c_int, C.c_int32, C.c_float] + [C.c_void_p] * 4

@@ -1,33 +1,16 @@
-"""ctypes binding of the new-map-point checker (oracle/new_points.mk).  TEST INFRASTRUCTURE, NOT PRODUCT.
+"""ctypes binding of the new-map-point checker (oracle/Makefile).  TEST INFRASTRUCTURE, NOT PRODUCT.
 
-  oracle(cur, neighbours, mutate=0)   oracle/libnew_points_oracle.so: the sequential loop of LocalMapping::CreateNewMapPoints over the
+  oracle(cur, neighbours, mutate=0)   oracle/liboracle.so (new_points_oracle.cpp): the sequential loop of LocalMapping::CreateNewMapPoints over the
                                       view dicts api.new_map_points reads -> (points, best2, verdict), shaped as api.new_map_points'
   svd4_null(A)                        the stated 4x4 decomposition alone: A (4,4) f32 -> vt.row(3)
 """
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_LIB = None
-
-
-def build() -> None:
-    subprocess.check_call(["make", "-C", _HERE, "-s", "-f", "new_points.mk", "ref"])
-
-
-def lib():
-    global _LIB
-    if _LIB is None:
-        so = os.path.join(_HERE, "libnew_points_oracle.so")
-        if not os.path.exists(so):
-            build()
-        _LIB = C.CDLL(so)
-    return _LIB
+from oracle import pyoracle
 
 
 def oracle(cur, neighbours, mutate=0, capacity=None):
@@ -40,7 +23,7 @@ def oracle(cur, neighbours, mutate=0, capacity=None):
     out = np.zeros(max(cap, 1), api.NEW_POINT_DTYPE)
     best2 = np.full((B, n), -2, np.int32); verdict = np.full((B, n), 255, np.uint8)
     n_out = C.c_int32(-1)
-    rc = lib().orc_new_map_points(C.byref(c), nbs, B, out.ctypes.data_as(C.c_void_p), cap, C.byref(n_out), best2.ctypes.data_as(C.c_void_p),
+    rc = pyoracle.lib().orc_new_map_points(C.byref(c), nbs, B, out.ctypes.data_as(C.c_void_p), cap, C.byref(n_out), best2.ctypes.data_as(C.c_void_p),
                                   verdict.ctypes.data_as(C.c_void_p), int(mutate))
     if rc != 0:
         raise ValueError("orc_new_map_points: capacity %d below the %d points needed" % (cap, n_out.value))
@@ -50,7 +33,7 @@ def oracle(cur, neighbours, mutate=0, capacity=None):
 def svd4_null(A):
     A = np.ascontiguousarray(A, np.float32).reshape(16)
     x = np.zeros(4, np.float32)
-    lib().orc_svd4_null(A.ctypes.data_as(C.c_void_p), x.ctypes.data_as(C.c_void_p))
+    pyoracle.lib().orc_svd4_null(A.ctypes.data_as(C.c_void_p), x.ctypes.data_as(C.c_void_p))
     return x
 
 
@@ -62,10 +45,7 @@ class StandIn:
 
     def __init__(self, cur, neighbours, median_depth=None, gpu=False):
         from ccm_slam_b200 import api
-        so = os.path.join(_HERE, "_ref", "libnew_points_shim_gpu.so" if gpu else "libnew_points_shim.so")
-        if not os.path.exists(so):
-            build()
-        self.L = C.CDLL(so)
+        self.L = pyoracle.ref_lib("libnew_points_shim_gpu.so" if gpu else "libnew_points_shim.so")
         self.L.np_scene_create.restype = C.c_void_p
         for f in ("np_scene_destroy", "np_point_count", "np_polls"):
             getattr(self.L, f).argtypes = [C.c_void_p]

@@ -449,28 +449,34 @@ class Vocabulary:
             lib().orc_voc_destroy(C.c_void_p(self.h)); self.h = None
 
 
-# ---- the reference's own DBoW2, compiled in place by `make -C oracle ref` (only where /root/reference exists) ---------------
-_REF_DBOW2 = None
+# ---- oracle/_ref/: the reference's own sources compiled in place, and the shims on stand-in classes (`make -C oracle ref`) ----------
+_REF_LIBS = {}
 
 
 def build_ref() -> str | None:
-    """oracle/_ref/libdbow2_ref.so from the reference's DBoW2 sources (nothing copied); None where the reference tree is absent
-    and no prebuilt library travelled with the repository."""
+    """`make ref`: whatever of oracle/_ref/ can be built here (the reference's own code only where its tree is present, the stand-in shims
+    only where the product library is); returns oracle/_ref/libdbow2_ref.so, None where it is absent."""
+    subprocess.check_call(["make", "-C", _HERE, "-s", "-j", str(min(8, os.cpu_count() or 1)), "ref"])
     so = os.path.join(_HERE, "_ref", "libdbow2_ref.so")
-    if os.path.isdir("/root/reference/cslam/thirdparty/DBoW2"):
-        subprocess.check_call(["make", "-C", _HERE, "-s", "-j", str(min(8, os.cpu_count() or 1)), "ref"])
     return so if os.path.exists(so) else None
 
 
-def ref_dbow2():
-    global _REF_DBOW2
-    if _REF_DBOW2 is None:
-        so = build_ref()
-        if so is None:
+def ref_lib(name):
+    """oracle/_ref/<name> after `make ref`, loaded once; None where it is absent"""
+    if name not in _REF_LIBS:
+        build_ref()
+        so = os.path.join(_HERE, "_ref", name)
+        if not os.path.exists(so):
             return None
-        _REF_DBOW2 = C.CDLL(so)
-        _REF_DBOW2.ref_voc_load.restype = C.c_void_p
-    return _REF_DBOW2
+        _REF_LIBS[name] = C.CDLL(so)
+    return _REF_LIBS[name]
+
+
+def ref_dbow2():
+    L = ref_lib("libdbow2_ref.so")
+    if L is not None:
+        L.ref_voc_load.restype = C.c_void_p
+    return L
 
 
 def ref_orb_cli():
@@ -500,34 +506,12 @@ def ref_orb_extract(img, cfg=None, allocator="bump"):
 
 
 # ---- the reference's own Levenberg-Marquardt driver on the oracle's linear algebra (oracle/_ref/liblm_ref.so) -------------------------
-_REF_LM = None
-
-
 def ref_lm():
-    global _REF_LM
-    if _REF_LM is None:
-        if build_ref() is None:
-            return None
-        so = os.path.join(_HERE, "_ref", "liblm_ref.so")
-        if not os.path.exists(so):
-            return None
-        _REF_LM = C.CDLL(so)
-    return _REF_LM
-
-
-_REF_BA_FULL = None
+    return ref_lib("liblm_ref.so")
 
 
 def ref_ba_full():
-    global _REF_BA_FULL
-    if _REF_BA_FULL is None:
-        if build_ref() is None:
-            return None
-        so = os.path.join(_HERE, "_ref", "libba_full_ref.so")
-        if not os.path.exists(so):
-            return None
-        _REF_BA_FULL = C.CDLL(so)
-    return _REF_BA_FULL
+    return ref_lib("libba_full_ref.so")
 
 
 def ref_ba_full_solve(p, **kw):
@@ -536,19 +520,8 @@ def ref_ba_full_solve(p, **kw):
     return ba_solve(p, fn=ref_ba_full().ref_ba_full_solve, **kw)
 
 
-_REF_BA_BLOCK = None
-
-
 def ref_ba_block():
-    global _REF_BA_BLOCK
-    if _REF_BA_BLOCK is None:
-        if build_ref() is None:
-            return None
-        so = os.path.join(_HERE, "_ref", "libba_block_ref.so")
-        if not os.path.exists(so):
-            return None
-        _REF_BA_BLOCK = C.CDLL(so)
-    return _REF_BA_BLOCK
+    return ref_lib("libba_block_ref.so")
 
 
 def ref_ba_block_solve(p, **kw):
@@ -565,19 +538,8 @@ def ref_ba_solve(p, **kw):
 
 
 # ---- g2o's own vertex / edge types, Lie groups and Huber kernel (oracle/_ref/libg2o_types_ref.so, oracle/ref_g2o_wrap.cpp) ---------------
-_REF_G2O = None
-
-
 def ref_g2o():
-    global _REF_G2O
-    if _REF_G2O is None:
-        if build_ref() is None:
-            return None
-        so = os.path.join(_HERE, "_ref", "libg2o_types_ref.so")
-        if not os.path.exists(so):
-            return None
-        _REF_G2O = C.CDLL(so)
-    return _REF_G2O
+    return ref_lib("libg2o_types_ref.so")
 
 
 class Pieces:
@@ -642,30 +604,14 @@ def ref_vertex_oplus(kind, est, upd, flag=0):
 
 
 # ---- the reference's own ORBmatcher.cpp on stand-in Frame / KeyFrame / MapPoint (oracle/_ref/libmatch_ref.so) -----------------------
-_REF_MATCH = None
-_SHIM_MATCH = {}
 _MATCH_SIDE = "ref"
 
 
 def ref_match():
     """the matcher library the ref_* wrappers below talk to: the reference's own ORBmatcher.cpp (default) or, inside
     `with matcher_side("shim")`, this repository's shim/ORBmatcher*_shim.cpp built over the same stand-in classes"""
-    global _REF_MATCH, _SHIM_MATCH
-    if _MATCH_SIDE in ("shim", "shim_gpu"):     # "shim": device half doubled on the CPU; "shim_gpu": the real device entry points
-        if _SHIM_MATCH.get(_MATCH_SIDE) is None:
-            so = os.path.join(_HERE, "_ref", "libmatch_shim.so" if _MATCH_SIDE == "shim" else "libmatch_shim_gpu.so")
-            if build_ref() is None or not os.path.exists(so):
-                return None
-            _SHIM_MATCH[_MATCH_SIDE] = C.CDLL(so)
-        return _SHIM_MATCH[_MATCH_SIDE]
-    if _REF_MATCH is None:
-        if build_ref() is None:
-            return None
-        so = os.path.join(_HERE, "_ref", "libmatch_ref.so")
-        if not os.path.exists(so):
-            return None
-        _REF_MATCH = C.CDLL(so)
-    return _REF_MATCH
+    # "shim": device half doubled on the CPU; "shim_gpu": the real device entry points
+    return ref_lib({"shim": "libmatch_shim.so", "shim_gpu": "libmatch_shim_gpu.so"}.get(_MATCH_SIDE, "libmatch_ref.so"))
 
 
 class matcher_side:
@@ -919,19 +865,8 @@ def sim3_opt_trace(S12, P1c, P2c, uv1, uv2, w1, w2, K1, K2, th2, fix_scale):
 
 
 # ---- the two single-vertex optimisations run by the reference's LM driver over the reference's vertices / edges (oracle/ref_single_full_wrap.cpp)
-_REF_SINGLE = None
-
-
 def ref_single_full():
-    global _REF_SINGLE
-    if _REF_SINGLE is None:
-        if build_ref() is None:
-            return None
-        so = os.path.join(_HERE, "_ref", "libsingle_full_ref.so")
-        if not os.path.exists(so):
-            return None
-        _REF_SINGLE = C.CDLL(so)
-    return _REF_SINGLE
+    return ref_lib("libsingle_full_ref.so")
 
 
 def ref_pose_optimize(*a):
@@ -943,38 +878,16 @@ def ref_sim3_optimize(*a):
 
 
 # ---- the essential graph run by the reference's LM driver over the reference's VertexSim3Expmap / EdgeSim3 (oracle/ref_pgo_full_wrap.cpp)
-_REF_PGO = None
-
-
 def ref_pgo_full():
-    global _REF_PGO
-    if _REF_PGO is None:
-        if build_ref() is None:
-            return None
-        so = os.path.join(_HERE, "_ref", "libpgo_full_ref.so")
-        if not os.path.exists(so):
-            return None
-        _REF_PGO = C.CDLL(so)
-    return _REF_PGO
+    return ref_lib("libpgo_full_ref.so")
 
 
 def ref_pgo_solve(p, **kw):
     return pgo_solve(p, fn=ref_pgo_full().ref_pgo_solve, **kw)
 
 
-_REF_PGO_BLOCK = None
-
-
 def ref_pgo_block():
-    global _REF_PGO_BLOCK
-    if _REF_PGO_BLOCK is None:
-        if build_ref() is None:
-            return None
-        so = os.path.join(_HERE, "_ref", "libpgo_block_ref.so")
-        if not os.path.exists(so):
-            return None
-        _REF_PGO_BLOCK = C.CDLL(so)
-    return _REF_PGO_BLOCK
+    return ref_lib("libpgo_block_ref.so")
 
 
 def ref_pgo_block_solve(p, **kw):

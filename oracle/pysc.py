@@ -1,6 +1,6 @@
-"""ctypes binding of the Sim3 correction checker (oracle/sim3_correction.mk).  TEST INFRASTRUCTURE, NOT PRODUCT.
+"""ctypes binding of the Sim3 correction checker (oracle/Makefile).  TEST INFRASTRUCTURE, NOT PRODUCT.
 
-  oracle(sc, fn=None)    oracle/libsim3_correction_oracle.so: the entries walked in order as LoopFinder::CorrectLoop /
+  oracle(sc, fn=None)    oracle/liboracle.so (sim3_correction_oracle.cpp): the entries walked in order as LoopFinder::CorrectLoop /
                          MapMerger::MergeMaps walk them, over the flat arrays of ccm_sim3_correction.  fn: any function with the
                          same C signature (the g++ build of the product's arithmetic in the tests) instead of the oracle
 Returns the outputs of ccm_slam_b200.api.sim3_correction.
@@ -8,32 +8,15 @@ Returns the outputs of ccm_slam_b200.api.sim3_correction.
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_LIB = None
-
-
-def build() -> None:
-    subprocess.check_call(["make", "-C", _HERE, "-s", "-f", "sim3_correction.mk", "ref"])
-
-
-def lib():
-    global _LIB
-    if _LIB is None:
-        so = os.path.join(_HERE, "libsim3_correction_oracle.so")
-        if not os.path.exists(so):
-            build()
-        _LIB = C.CDLL(so)
-    return _LIB
+from oracle import pyoracle
 
 
 def oracle(sc, fn=None):
     from ccm_slam_b200 import api
     out = api.sim3_correction_out(len(sc["entry_kf"]), len(sc["mp_skip"]))
     argv, _keep = api.sim3_correction_args(sc, out)
-    rc = (fn or lib().orc_sim3_correction)(*argv)
+    rc = (fn or pyoracle.lib().orc_sim3_correction)(*argv)
     if rc != 0:
         raise ValueError("orc_sim3_correction: bad input")
     return out
@@ -45,7 +28,7 @@ class StandIn:
     ccm_sim3_correction, or the real library with gpu=True.  The scene must give every observed point a reference keyframe."""
 
     def __init__(self, sc, gpu=False):
-        self.L = C.CDLL(os.path.join(_HERE, "_ref", "libsim3_correction_shim_gpu.so" if gpu else "libsim3_correction_shim.so"))
+        self.L = pyoracle.ref_lib("libsim3_correction_shim_gpu.so" if gpu else "libsim3_correction_shim.so")
         self.L.sc_scene_create.restype = C.c_void_p
         self.L.sc_scene_destroy.argtypes = [C.c_void_p]
         self.L.sc_literal.argtypes = [C.c_void_p, C.c_int]

@@ -1,6 +1,6 @@
-"""ctypes binding of the loop / merge fusion checker (oracle/search_and_fuse.mk).  TEST INFRASTRUCTURE, NOT PRODUCT.
+"""ctypes binding of the loop / merge fusion checker (oracle/Makefile).  TEST INFRASTRUCTURE, NOT PRODUCT.
 
-  oracle(sc)   oracle/libsearch_and_fuse_oracle.so: every (corrected keyframe, loop point) pair LoopFinder / MapMerger::SearchAndFuse
+  oracle(sc)   oracle/liboracle.so (search_and_fuse_oracle.cpp): every (corrected keyframe, loop point) pair LoopFinder / MapMerger::SearchAndFuse
                searches, Fuse(Scw)'s prelude with the host's logf and the reference-pinned window search, over a scene as
                synth_match.make_search_and_fuse_scene builds it -> best (K, P), shaped as api.search_and_fuse's first result.
                th, chi2, camera and skip select the wrong variants the tests must tell apart from the real one.
@@ -8,27 +8,10 @@
 from __future__ import annotations
 
 import ctypes as C
-import os
-import subprocess
 
 import numpy as np
 
-_HERE = os.path.dirname(os.path.abspath(__file__))
-_LIB = None
-
-
-def build() -> None:
-    subprocess.check_call(["make", "-C", _HERE, "-s", "-f", "search_and_fuse.mk", "ref"])
-
-
-def lib():
-    global _LIB
-    if _LIB is None:
-        so = os.path.join(_HERE, "libsearch_and_fuse_oracle.so")
-        if not os.path.exists(so):
-            build()
-        _LIB = C.CDLL(so)
-    return _LIB
+from oracle import pyoracle
 
 
 def oracle(sc, th=4.0, chi2=False, camera="split", skip="skip"):
@@ -39,7 +22,7 @@ def oracle(sc, th=4.0, chi2=False, camera="split", skip="skip"):
     T, O = ("Tcw", "Ow") if camera == "split" else ("Tcw_pose", "Ow_pose")
     kfs, K, pts = api.search_and_fuse_structs(sc, keep, T, O, skip)
     best = np.full((K, pts.n), -3, np.int32)
-    lib().orc_search_and_fuse(kfs, K, C.byref(pts), C.c_float(th), int(chi2), best.ctypes.data_as(C.c_void_p))
+    pyoracle.lib().orc_search_and_fuse(kfs, K, C.byref(pts), C.c_float(th), int(chi2), best.ctypes.data_as(C.c_void_p))
     return best
 
 
@@ -51,10 +34,7 @@ class StandIn:
 
     def __init__(self, sc, gpu=False, empty_kf=()):
         from ccm_slam_b200 import api
-        so = os.path.join(_HERE, "_ref", "libsearch_and_fuse_shim_gpu.so" if gpu else "libsearch_and_fuse_shim.so")
-        if not os.path.exists(so):
-            build()
-        self.L = C.CDLL(so)
+        self.L = pyoracle.ref_lib("libsearch_and_fuse_shim_gpu.so" if gpu else "libsearch_and_fuse_shim.so")
         self.L.sf_scene_create.restype = C.c_void_p
         self.L.sf_scene_destroy.argtypes = [C.c_void_p]
         self.L.sf_run.argtypes = [C.c_void_p, C.c_int, C.c_int]

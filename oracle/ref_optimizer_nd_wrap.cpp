@@ -1,5 +1,5 @@
 // ref_optimizer_nd_wrap.cpp — TEST INFRASTRUCTURE: what the five write-back loops of shim/Optimizer_shim.cpp leave in the map points
-// when shim/MapPoint_shim.cpp is linked next to it (oracle/normal_depth.mk: _ref/liboptimizer_nd_shim{,_gpu}.so).
+// when shim/MapPoint_shim.cpp is linked next to it (oracle/Makefile: _ref/liboptimizer_nd_shim{,_gpu}.so).
 //
 // The optimiser calls themselves are ref_optimizer_wrap.cpp's (optw_gba, optw_gba_mirror, optw_local_ba, optw_essential_graph), linked
 // unchanged into the same library over the stand-ins of ref_stub_opt_mp.  Their scene is destroyed when they return; each MapPoint

@@ -3,13 +3,13 @@
 // of ccm_sim3_correction (include/ccm_b200.h).  Written from the reference loop, not from the product's sim3_correction_math.cuh:
 // it walks the entries in order exactly as the reference does, keeps a live table of camera centres, moves and tags each point the
 // moment an entry reaches it, runs UpdateNormalAndDepth on it against the centres as they stand at that moment (orc_normal_depth of
-// libnormal_depth_oracle.so, one point at a time), and overwrites the entry's centre only after its points.  Which entry claims a
+// normal_depth_oracle.cpp, one point at a time), and overwrites the entry's centre only after its points.  Which entry claims a
 // point and which centres its normal sees are therefore outcomes of the walk, not assumptions.
 //   g2o::Sim3::map       s*(r*x) + t, r*x = Eigen's _transformVector: uv = 2 (q.vec x v); v + w uv + q.vec x uv
 //   g2o::Sim3::inverse   (r.conjugate(), r.conjugate() * ((-1./s) * t), 1./s)
 //   toRotationMatrix     Eigen's Quaternion::toRotationMatrix
 //   eigt *= (1./s); toCvSE3; SetPose: Ow = -Rcw^T tcw summed left to right in f32
-// Compiled by oracle/sim3_correction.mk with -ffp-contract=off.
+// Compiled by oracle/Makefile with -ffp-contract=off.
 #include <cstdint>
 #include <vector>
 

@@ -2,7 +2,7 @@
 (cslam/src/KeyFrame.cpp:629-711) on hand-made edge cases, tie storms and random scenes.  The fixture stores each case's inputs (the
 keys of synth.make_covisibility) and the answer in the flat layout of ccm_covisibility (conn_ptr, conn_kf, conn_w, n_sel, sel_kf,
 sel_w, status).  The answer is the pure-Python witness below (a dict per keyframe, sorted()); the generator refuses to write unless
-the oracle (oracle/libcovis_oracle.so) agrees on every case.  Run from the repo root:
+the oracle (oracle/covis_oracle.cpp) agrees on every case.  Run from the repo root:
     python tests/golden/make_covisibility_golden.py
 """
 import os

@@ -6,7 +6,7 @@ and MapPoint::SetBadFlag (which nulls the point in every observer's slots) and c
 
 The f64 / f32 case is found by search: the first (threshold, nMPs, nRedundant) in a fixed order for which `nRed > thres * nMPs` in
 f64 and the same expression in f32 disagree (none exists for 0.98 below 5000 points).  Before it writes, every case is checked against
-the oracle (oracle/libkeyframe_culling_oracle.so); the generator refuses to write on any difference.  Inputs and outputs are both
+the oracle (oracle/keyframe_culling_oracle.cpp); the generator refuses to write on any difference.  Inputs and outputs are both
 stored, so the fixture does not depend on the generator's random streams.  Run from the repo root:
     python tests/golden/make_keyframe_culling_golden.py
 """

@@ -6,7 +6,7 @@ synth.make_sim3_correction.  The witness walks the entries in map order as the r
     UpdateNormalAndDepth()                              the cv2 evaluation of make_normal_depth_golden.py, against the live centres
     R, t *= (1./s), toCvSE3                             f64, then each element to f32
     SetPose: Ow = -Rwc * tcw                            cv2.gemm on the f32 matrices
-Before it writes, every output is checked against the oracle (oracle/libsim3_correction_oracle.so); the generator refuses to write on
+Before it writes, every output is checked against the oracle (oracle/sim3_correction_oracle.cpp); the generator refuses to write on
 any difference.  Inputs and outputs are both stored, so the fixture does not depend on the generator's random streams.  Run from the
 repo root (cv2 4.13):
     python tests/golden/make_sim3_correction_golden.py

@@ -1,4 +1,4 @@
-"""CPU suite: shim/KeyFrameConnections_shim.cpp over the CPU double of the device entry point (oracle/covis.mk).
+"""CPU suite: shim/KeyFrameConnections_shim.cpp over the CPU double of the device entry point (oracle/Makefile).
 
  * a MergeMaps-shaped loop (per keyframe SetPose + UpdateConnections) leaves every keyframe's mConnectedKeyFrameWeights, ordered
    list and weights, parent and children exactly as the literal restatement does, through the parked path (one device call, one hit

@@ -1,4 +1,4 @@
-"""CPU suite: shim/MapPointDescriptor_shim.cpp over the CPU doubles of the device entry points (oracle/distinctive.mk).
+"""CPU suite: shim/MapPointDescriptor_shim.cpp over the CPU doubles of the device entry points (oracle/Makefile).
 
  * on fresh scenes the parked path (ccm_b200_prepare_descriptors + the member) and the host path leave identical mDescriptor members:
    bytes, type and shape; one parked choice is taken per written point; the store variant of the preparation gives the same;

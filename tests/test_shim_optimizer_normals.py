@@ -1,4 +1,4 @@
-"""The five write-back loops of shim/Optimizer_shim.cpp with shim/MapPoint_shim.cpp linked next to them (oracle/normal_depth.mk:
+"""The five write-back loops of shim/Optimizer_shim.cpp with shim/MapPoint_shim.cpp linked next to them (oracle/Makefile:
 _ref/liboptimizer_nd_shim.so, device entry points doubled on the CPU; the GPU build is driven from tests/test_gpu_normal_depth.py).
 
 For MapFusionGBA (direct and through a registered mirror), GlobalBundleAdjustemntClient, LocalBundleAdjustmentClient and both
@@ -21,10 +21,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 def nd_lib(gpu):
     so = os.path.join(HERE, "..", "oracle", "_ref", "liboptimizer_nd_shim_gpu.so" if gpu else "liboptimizer_nd_shim.so")
     if not os.path.exists(so):
-        from oracle import pyoracle, pynd
+        from oracle import pyoracle
         if pyoracle.build_ref() is None:
             return None
-        pynd.build()
     return C.CDLL(so) if os.path.exists(so) else None
 
 

@@ -24,7 +24,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 from ccm_slam_b200 import api  # noqa: E402
 from ccm_slam_b200 import synth_match as sm  # noqa: E402
-from oracle import pyfn  # noqa: E402
+from oracle import pyoracle  # noqa: E402
 
 
 def queries(k, pts, rows):
@@ -101,7 +101,7 @@ def main():
         for i, e in enumerate(sc["entries"]):
             api._chk(L.ccm_fuse_search(C.byref(G[e]), C.byref(Qe[i]), api._p(il[e]), len(il[e]), api._p(best_e[i]), C.byref(nf)))
         api._chk(L.ccm_fuse_search(C.byref(Gc), C.byref(Qb), api._p(il[-1]), len(il[-1]), api._p(best_b), C.byref(nf)))
-    olib = pyfn.lib()
+    olib = pyoracle.lib()
     of = np.zeros((T, n), np.int32); ob = np.zeros(nc, np.int32)
 
     def call_c():

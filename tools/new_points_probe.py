@@ -49,16 +49,16 @@ class Prebuilt:
         return self.out[:self.n_out.value].copy()
 
     def oracle(self):
-        from oracle import pynp
-        rc = pynp.lib().orc_new_map_points(C.byref(self.cur), self.nbs, self.B, api._p(self.out), len(self.out), C.byref(self.n_out), None, None, 0)
+        from oracle import pyoracle
+        rc = pyoracle.lib().orc_new_map_points(C.byref(self.cur), self.nbs, self.B, api._p(self.out), len(self.out), C.byref(self.n_out), None, None, 0)
         assert rc == 0
         return self.out[:self.n_out.value].copy()
 
     def per_pair(self, match):
         """(b): per neighbour, `match` = ccm_match_triangulation, then the oracle's triangulation of exactly those pairs (the oracle over
         that neighbour alone with every other feature masked), the accepted features folded into has_mp for the next neighbour"""
-        from oracle import pynp
-        tri = pynp.lib().orc_new_map_points
+        from oracle import pyoracle
+        tri = pyoracle.lib().orc_new_map_points
         self.has[:] = self.has0
         got = []
         npairs = C.c_int32()

@@ -29,7 +29,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 from ccm_slam_b200 import api  # noqa: E402
 from ccm_slam_b200 import synth_match as sm  # noqa: E402
-from oracle import pysf  # noqa: E402
+from oracle import pyoracle, pysf  # noqa: E402
 from tools.fuse_probe import queries, timed  # noqa: E402
 
 SHAPES = {"loop": dict(n_kf=31, n=1000, n_loop=8000), "stress": dict(n_kf=100, n=1000, n_loop=30000)}
@@ -65,7 +65,7 @@ def run(shape, reps):
 
     def call_h():
         api._chk(L.ccm_search_and_fuse_host(kfs, K, C.byref(pts), api._p(hbest), None))
-    olib = pysf.lib()
+    olib = pyoracle.lib()
 
     def call_c():
         olib.orc_search_and_fuse(kfs, K, C.byref(pts), C.c_float(4.0), 0, api._p(obest))
