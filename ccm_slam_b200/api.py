@@ -280,6 +280,15 @@ class BAHandle:
         _chk(lib().ccm_ba_debug_schur_blocks(self._h, _p(rowptr), _p(col), _p(val), _p(bs)))
         return dict(rowptr=rowptr, col=col[:nnzb], val=val[:nnzb], bschur=bs)
 
+    def debug_products(self):
+        """the Schur product lists (ccm_ba_debug_products): blk (nub, 2) upper blocks as (row, column) pose indices, ptr (nub+1,)
+        list offsets, pairs (nprod, 2) observation pairs (e, o) as positions in the landmark-sorted observation order"""
+        i = self.info()
+        nub, nprod = i["s_blocks_upper"], i["schur_products"]
+        blk = np.empty((max(nub, 1), 2), np.int32); ptr = np.empty(nub + 1, np.uint32); pairs = np.empty((max(nprod, 1), 2), np.int32)
+        _chk(lib().ccm_ba_debug_products(self._h, _p(blk), _p(ptr), _p(pairs)))
+        return dict(blk=blk[:nub], ptr=ptr.astype(np.int64), pairs=pairs[:nprod])
+
     PATH_KEYS = ("pcg_impl", "pcg_block", "pcg_agg", "pcg_nc")
 
     def debug_paths(self):

@@ -409,30 +409,36 @@ __global__ void __launch_bounds__(1024) k_sum_partials(const double* __restrict_
 // entry -> row dependence costs one memory latency per batch instead of two.  On H100 the kernel is bound by the rows it keeps in
 // flight: the 2 * UNROLL rows of a batch are requested together, and UNROLL 16 at 66 registers runs a cfg5 launch in 9.6 ms against
 // 11.3 at UNROLL 8 (48 registers), 10.0 at 32 and 12.7 at 4 (H100 80GB HBM3, 700 W).  (dmma_884: pcg.cuh)
-// The explicit minimum of one CTA per SM in the launch bounds lets ptxas hold every row of a batch in its own registers (96, five
-// CTAs = 20 warps per SM) instead of squeezing the batch into 66 (seven CTAs): fewer warps, but each keeps all 32 rows of its batch in
-// flight, and a cfg5 launch takes 8.3-8.6 ms against 9.5.  Capping it at 64 registers for 32 warps per SM (128, 64, 32 or 256-thread
-// CTAs) gives 9.7-10.9 ms (H100 80GB HBM3, 700 W).
-
-constexpr int SCHUR_CTA = 128;   // threads per CTA of k_schur_mma: 4 upper blocks
-__global__ void __launch_bounds__(SCHUR_CTA, 1) k_schur_mma(const uint2* __restrict__ prod, const unsigned* __restrict__ u_prod_ptr,
-                                                         const int* __restrict__ u_row, const int* __restrict__ u_col, int nub,
-                                                         const double* __restrict__ Z, const int* __restrict__ o_lm,
-                                                         const double* __restrict__ gvec, double* __restrict__ U_val,
-                                                         double* __restrict__ bneg) {
+// Holding every row of a batch in its own registers (96, 20 warps per SM) beats squeezing the batch into 66 registers (28 warps): fewer
+// warps, but each keeps all 32 rows of its batch in flight, and a cfg5 launch took 8.3-8.6 ms against 9.5 (128-thread CTAs).  Capping
+// it at 64 registers for 32 warps per SM (128, 64, 32 or 256-thread CTAs) gives 9.7-10.9 ms (H100 80GB HBM3, 700 W).
+//
+// Schedule: one CTA of SCHUR_WARPS warps per SM.  The upper blocks of a block row share its a-side rows of Z, so they run on one SM
+// at the same time, and since every list is in landmark order (k_row_products) they walk those rows in the same direction: the
+// a-side fetches of a row's blocks meet in L1.  The work is a row-major sequence of tasks (a task: the upper blocks of one row,
+// longest list first; a row of more than SCHUR_TASK blocks is cut into several tasks, so that one long row - a loop closure, a
+// merged map - cannot serialise the end of the launch).  CTAs take tasks from a global counter in order, which keeps the rows in
+// progress across the device as narrow as with one warp per block; a CTA's warps take the blocks of its current task from a
+// shared counter, and the warp that exhausts it takes the next task for the CTA while the others finish their blocks: no barrier.
+// A cfg5 launch takes 7.5-7.9 ms against 8.3-8.7 with one warp per block and four blocks per CTA; two adjacent rows per task
+// (tasks of up to 128 blocks) take 9.0 (H100 80GB HBM3, 700 W).
+constexpr int SCHUR_WARPS = 20;                 // 640 threads x 96 registers fill the register file: the warps per SM of 5 x 128
+constexpr int SCHUR_CTA = SCHUR_WARPS * 32;
+constexpr int SCHUR_TASK = 64;                  // most blocks of one task
+__device__ __forceinline__ void schur_block(int u, int lane, const uint2* __restrict__ prod, const unsigned* __restrict__ u_prod_ptr,
+                                            const int* __restrict__ u_row, const int* __restrict__ u_col,
+                                            const double* __restrict__ Z, const int* __restrict__ o_lm,
+                                            const double* __restrict__ gvec, double* __restrict__ U_val, double* __restrict__ bneg) {
   constexpr int UNROLL = 16;  // products per batch; even: they alternate between the two accumulator sets; <= 32 (one entry per lane)
-  const int warp = (int)(((long long)blockIdx.x * SCHUR_CTA + threadIdx.x) >> 5);
-  if (warp >= nub) return;  // warp-uniform
-  const int lane = threadIdx.x & 31;
   const int m = lane >> 2, k = lane & 3;
   const bool ld = m < 6 && k < 3;
   constexpr int zs = 18;   // doubles per row of Z.  Padded rows (a 128-byte line per half-warp, 160 / 192 / 256-byte strides) were measured
                            // and are no faster
   // padding lanes read an element their own half-warp reads anyway (no extra line) and discard it
   const int off = ld ? m * 3 + k : (lane < 16 ? 0 : 12);
-  const unsigned beg = u_prod_ptr[warp], end = u_prod_ptr[warp + 1];
-  const int row = u_row[warp];
-  const bool diag = row == u_col[warp];
+  const unsigned beg = u_prod_ptr[u], end = u_prod_ptr[u + 1];
+  const int row = u_row[u];
+  const bool diag = row == u_col[u];
   double c00 = 0.0, c01 = 0.0, c10 = 0.0, c11 = 0.0;
   unsigned p = beg;
   if (!diag) {
@@ -498,10 +504,39 @@ __global__ void __launch_bounds__(SCHUR_CTA, 1) k_schur_mma(const uint2* __restr
   }
   c00 += c10; c01 += c11;
   if (ld) {
-    U_val[(size_t)warp * 36 + m * 6 + 2 * k] = -c00;
-    U_val[(size_t)warp * 36 + m * 6 + 2 * k + 1] = -c01;
+    U_val[(size_t)u * 36 + m * 6 + 2 * k] = -c00;
+    U_val[(size_t)u * 36 + m * 6 + 2 * k + 1] = -c01;
   }
   if (diag && m < 6 && k == 3) bneg[(size_t)row * 6 + m] = -c00;  // C[m][6]
+}
+
+// task_ptr [ntasks+1]: each task's range in u_sched (the upper blocks, row-major, longest list first within a row); next_task: 0
+// before the launch
+__global__ void __launch_bounds__(SCHUR_CTA, 1) k_schur_mma(const uint2* __restrict__ prod, const unsigned* __restrict__ u_prod_ptr,
+                                                         const int* __restrict__ u_row, const int* __restrict__ u_col,
+                                                         const int* __restrict__ u_sched, const int* __restrict__ task_ptr,
+                                                         int ntasks, int* __restrict__ next_task, const double* __restrict__ Z,
+                                                         const int* __restrict__ o_lm, const double* __restrict__ gvec,
+                                                         double* __restrict__ U_val, double* __restrict__ bneg) {
+  __shared__ unsigned long long s_state;   // (current task << 32) | blocks of it handed out
+  const int lane = threadIdx.x & 31;
+  if (threadIdx.x == 0) s_state = (unsigned long long)atomicAdd(next_task, 1) << 32;
+  __syncthreads();
+  for (;;) {
+    unsigned long long st = 0;
+    if (lane == 0) st = atomicAdd(&s_state, 1ull);
+    st = __shfl_sync(0xffffffffu, st, 0);
+    const int t = (int)(st >> 32), i = (int)(unsigned)st;
+    if (t >= ntasks) break;
+    const int b0 = __ldg(task_ptr + t), n = __ldg(task_ptr + t + 1) - b0;
+    if (i < n) {
+      schur_block(__ldg(u_sched + b0 + i), lane, prod, u_prod_ptr, u_row, u_col, Z, o_lm, gvec, U_val, bneg);
+    } else if (lane == 0) {
+      if (i == n) atomicExch(&s_state, (unsigned long long)atomicAdd(next_task, 1) << 32);   // this warp moves the CTA on
+      else while ((int)(*(volatile unsigned long long*)&s_state >> 32) == t) {}            // wait until that is done
+    }
+    __syncwarp();
+  }
 }
 
 // S (full block-CSR) from the upper blocks: diagonal gets Hpp + lambda I, lower blocks are transposed copies.
@@ -793,26 +828,76 @@ __global__ void __launch_bounds__(TPB) k_unit_ptr(const int* __restrict__ head, 
   if (i == n - 1) units[rank[i]] = n;
 }
 
-// count (fill == 0) or fill (fill == 1) the product lists of the upper blocks; one thread per local observation
-__global__ void __launch_bounds__(TPB) k_products(const int* __restrict__ o_kf, const int* __restrict__ o_lm,
-                                                  const int* __restrict__ lm_ptr, const int* __restrict__ pose_slot,
-                                                  const unsigned* __restrict__ bitmap, const int* __restrict__ word_prefix,
-                                                  const int* __restrict__ s_rowptr, const int* __restrict__ csr_u, int words,
-                                                  int E, int fill, unsigned* __restrict__ counters,
-                                                  const unsigned* __restrict__ u_prod_ptr, uint2* __restrict__ prod) {
-  const long long e = (long long)blockIdx.x * TPB + threadIdx.x;
+// Row key of every local observation for the stable grouping by block row: its pose slot, Kf for a fixed pose (sorted past the rows)
+__global__ void __launch_bounds__(TPB) k_row_keys(const int* __restrict__ o_kf, const int* __restrict__ pose_slot, int E, int Kf,
+                                                  int* __restrict__ key, int* __restrict__ idx) {
+  const int e = blockIdx.x * TPB + threadIdx.x;
   if (e >= E) return;
   const int a = pose_slot[o_kf[e]];
-  if (a < 0) return;
-  const int lm = o_lm[e];
-  const int beg = lm_ptr[lm], end = lm_ptr[lm + 1];
-  for (int o = beg; o < end; o++) {
-    const int b = pose_slot[o_kf[o]];
-    if (b < a || (b == a && o != (int)e)) continue;
-    const int u = csr_u[csr_pos(bitmap, word_prefix, s_rowptr, words, a, b)];
-    const unsigned slot = atomicAdd(counters + u, 1u);
-    if (fill) prod[u_prod_ptr[u] + slot] = make_uint2((unsigned)e, (unsigned)o);
+  key[e] = a < 0 ? Kf : a;
+  idx[e] = e;
+}
+
+// Count (fill == 0) or fill (fill == 1) the product lists of the upper blocks of block row a, one warp per row.  The warp walks
+// row a's observations e in increasing order (landmark order: row_obs is a stable grouping of the observations by row), with the
+// lanes over the observations o of e's landmark; every pair (e, o) with row(o) > a, and (e, e), goes to block (a, row(o)) at that
+// block's cursor.  Only this warp touches row a's cursors, so they need no atomics, and every list comes out in increasing (e, o)
+// order: deterministic by construction.  Lanes that hit the same block in one step (a keyframe observing a landmark twice) take
+// consecutive slots in lane order.  A row of at most ROWP_CUR upper blocks keeps its cursors in shared memory, a longer one in
+// cursor[] (zero before each pass); the count pass leaves every block's count in cursor[], the fill writes at u_prod_ptr[u] + slot.
+constexpr int ROWP_CUR = 512;
+__global__ void __launch_bounds__(128) k_row_products(const int* __restrict__ row_obs, const int* __restrict__ row_obs_ptr, int Kf,
+                                                      const int* __restrict__ o_kf, const int* __restrict__ o_lm,
+                                                      const int* __restrict__ lm_ptr, const int* __restrict__ pose_slot,
+                                                      const unsigned* __restrict__ bitmap, const int* __restrict__ word_prefix,
+                                                      const int* __restrict__ s_rowptr, const int* __restrict__ s_diag,
+                                                      const int* __restrict__ u_diag, int nub, int words, int fill, unsigned* cursor,
+                                                      const unsigned* __restrict__ u_prod_ptr, uint2* __restrict__ prod) {
+  __shared__ unsigned s_cur[4][ROWP_CUR];
+  const int a = (int)(((long long)blockIdx.x * 128 + threadIdx.x) >> 5);
+  if (a >= Kf) return;  // warp-uniform
+  const int lane = threadIdx.x & 31;
+  const unsigned below = (1u << lane) - 1u;
+  const int ua = u_diag[a], nu = (a + 1 < Kf ? u_diag[a + 1] : nub) - ua;
+  const bool sh = nu <= ROWP_CUR;
+  unsigned* cur = sh ? s_cur[threadIdx.x >> 5] : cursor + ua;   // cursor of upper block ua + i: cur[i]
+  if (sh)
+    for (int i = lane; i < nu; i += 32) cur[i] = 0u;
+  __syncwarp();
+  const int q0 = s_diag[a];   // CSR position of block ua
+  const int rb = row_obs_ptr[a], re = row_obs_ptr[a + 1];
+  for (int c0 = rb; c0 < re; c0 += 32) {
+    // 32 observations of the row, their landmarks' observation ranges loaded together, then walked one by one
+    int ce = 0, cb = 0, cn = 0;
+    if (c0 + lane < re) {
+      ce = row_obs[c0 + lane];
+      const int lm = o_lm[ce];
+      cb = lm_ptr[lm]; cn = lm_ptr[lm + 1];
+    }
+    const int nc = min(32, re - c0);
+    for (int j = 0; j < nc; j++) {
+      const int e = __shfl_sync(0xffffffffu, ce, j), beg = __shfl_sync(0xffffffffu, cb, j), end = __shfl_sync(0xffffffffu, cn, j);
+      for (int o0 = beg; o0 < end; o0 += 32) {
+        const int o = o0 + lane;
+        int i = -1;
+        if (o < end) {
+          const int b = pose_slot[o_kf[o]];
+          if (b > a || o == e) i = csr_pos(bitmap, word_prefix, s_rowptr, words, a, b) - q0;
+        }
+        const unsigned grp = __match_any_sync(0xffffffffu, i);
+        unsigned base = 0;
+        if (i >= 0) {
+          base = cur[i];
+          if (fill) prod[u_prod_ptr[ua + i] + base + __popc(grp & below)] = make_uint2((unsigned)e, (unsigned)o);
+        }
+        __syncwarp();   // every lane of a group has read the cursor before its first lane moves it
+        if (i >= 0 && (grp & below) == 0u) cur[i] = base + __popc(grp);
+        __syncwarp();   // and the new value is visible to the next step's reads
+      }
+    }
   }
+  if (sh && !fill)
+    for (int i = lane; i < nu; i += 32) cursor[ua + i] = cur[i];
 }
 
 // validation of the caller's observation arrays: flags[0] |= out-of-range / negative weight, flags[1] |= not grouped by landmark

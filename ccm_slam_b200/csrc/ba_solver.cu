@@ -12,6 +12,7 @@
 #include <limits>
 #include <numeric>
 
+#include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
 
 #include "ba_kernels.cuh"
@@ -76,6 +77,8 @@ struct ccm_ba_handle {
   DevBuf<int> s_rowptr, s_col, s_row, s_diag, csr_u, u_row, u_col, u_diag, word_prefix;
   DevBuf<unsigned> bitmap, u_prod_ptr;
   DevBuf<uint2> prod;
+  DevBuf<int> u_sched, task_ptr, next_task;   // k_schur_mma's schedule: upper blocks by row, longest list first, cut into tasks
+  int ntasks = 0, schur_grid = 1;
   DevBuf<float4> kobs;            // per free pose: (u, v, signed w, landmark) of its observations, packed
   DevBuf<unsigned> kobs_ptr;
   // pcg
@@ -242,10 +245,12 @@ void step_z(ccm_ba_handle* h, int robust, double delta, double lambda) {
   launch_linearize(h, robust, delta, LIN_Z, lambda);
 }
 
-// K4: the Schur products, one warp per upper block (k_schur_mma)
+// K4: the Schur products, one warp per upper block, the blocks of a row on one SM (k_schur_mma)
 void launch_schur(ccm_ba_handle* h, cudaStream_t s) {
-  k_schur_mma<<<div_up((long long)h->nub * 32, SCHUR_CTA), SCHUR_CTA, 0, s>>>(h->prod.p, h->u_prod_ptr.p, h->u_row.p, h->u_col.p, h->nub,
-                                                                             h->Z.p, h->o_lm.p, h->gvec.p, h->U_val(), h->bneg());
+  if (h->ntasks == 0) return;
+  CCM_CUDA(cudaMemsetAsync(h->next_task.p, 0, sizeof(int), s));
+  k_schur_mma<<<h->schur_grid, SCHUR_CTA, 0, s>>>(h->prod.p, h->u_prod_ptr.p, h->u_row.p, h->u_col.p, h->u_sched.p, h->task_ptr.p,
+                                                  h->ntasks, h->next_task.p, h->Z.p, h->o_lm.p, h->gvec.p, h->U_val(), h->bneg());
 }
 
 void step_schur(ccm_ba_handle* h) {
@@ -737,16 +742,33 @@ void build(ccm_ba_handle* h, const ccm_ba_problem* p) {
   const int nub = h->nub;
 
   lap("pattern, upper index");
-  // ---- Schur product lists (local shard)
-  DevBuf<unsigned> counters; counters.alloc_zero(std::max(nub, 1), s);
+  // ---- Schur product lists (local shard), in landmark order: the local observations grouped by block row (a stable radix sort keeps
+  // landmark order inside a row), then one warp per row counts, and after the scan fills, its blocks' lists (k_row_products)
   std::vector<unsigned> h_pp((size_t)nub + 1, 0);
+  DevBuf<unsigned> cursor; cursor.alloc_zero(std::max(nub, 1), s);
+  DevBuf<int> row_obs, row_obs_ptr;
   if (El && nub) {
-    k_products<<<div_up(El, TPB), TPB, 0, s>>>(h->o_kf.p, h->o_lm.p, h->lm_ptr.p, h->pose_slot.p, h->bitmap.p,
-                                               h->word_prefix.p, h->s_rowptr.p, h->csr_u.p, words, El, 0, counters.p,
-                                               nullptr, nullptr);
+    {
+      DevBuf<int> key, idx, key_s;
+      key.alloc(El); idx.alloc(El); key_s.alloc(El); row_obs.alloc(El); row_obs_ptr.alloc((size_t)Kf + 1);
+      k_row_keys<<<div_up(El, TPB), TPB, 0, s>>>(h->o_kf.p, h->pose_slot.p, El, Kf, key.p, idx.p);
+      CCM_LAUNCHED();
+      int bits = 1;
+      while ((1ll << bits) <= Kf) bits++;
+      size_t tb = 0;
+      CCM_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, key.p, key_s.p, idx.p, row_obs.p, El, 0, bits, s));
+      DevBuf<unsigned char> tmp; tmp.alloc(tb + 16);
+      CCM_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tb, key.p, key_s.p, idx.p, row_obs.p, El, 0, bits, s));
+      k_lm_ptr<<<div_up((long long)Kf + 1, TPB), TPB, 0, s>>>(key_s.p, El, Kf, row_obs_ptr.p);   // first observation of each row
+      CCM_LAUNCHED();
+      CCM_CUDA(cudaStreamSynchronize(s));   // the temporaries die here
+    }
+    k_row_products<<<div_up((long long)Kf * 32, 128), 128, 0, s>>>(row_obs.p, row_obs_ptr.p, Kf, h->o_kf.p, h->o_lm.p, h->lm_ptr.p,
+                                                                   h->pose_slot.p, h->bitmap.p, h->word_prefix.p, h->s_rowptr.p,
+                                                                   h->s_diag.p, h->u_diag.p, nub, words, 0, cursor.p, nullptr, nullptr);
     CCM_LAUNCHED();
     std::vector<unsigned> c(nub);
-    counters.download(c.data(), nub, s);
+    cursor.download(c.data(), nub, s);
     CCM_CUDA(cudaStreamSynchronize(s));
     unsigned long long run = 0;
     for (int u = 0; u < nub; u++) { h_pp[u] = (unsigned)run; run += c[u]; }
@@ -757,11 +779,37 @@ void build(ccm_ba_handle* h, const ccm_ba_problem* p) {
   upload_vec(h->u_prod_ptr, h_pp, s);
   h->prod.alloc(std::max<long long>(h->nprod, 1));
   if (h->nprod) {
-    CCM_CUDA(cudaMemsetAsync(counters.p, 0, sizeof(unsigned) * nub, s));
-    k_products<<<div_up(El, TPB), TPB, 0, s>>>(h->o_kf.p, h->o_lm.p, h->lm_ptr.p, h->pose_slot.p, h->bitmap.p,
-                                               h->word_prefix.p, h->s_rowptr.p, h->csr_u.p, words, El, 1, counters.p,
-                                               h->u_prod_ptr.p, h->prod.p);
+    CCM_CUDA(cudaMemsetAsync(cursor.p, 0, sizeof(unsigned) * nub, s));
+    k_row_products<<<div_up((long long)Kf * 32, 128), 128, 0, s>>>(row_obs.p, row_obs_ptr.p, Kf, h->o_kf.p, h->o_lm.p, h->lm_ptr.p,
+                                                                   h->pose_slot.p, h->bitmap.p, h->word_prefix.p, h->s_rowptr.p,
+                                                                   h->s_diag.p, h->u_diag.p, nub, words, 1, cursor.p, h->u_prod_ptr.p,
+                                                                   h->prod.p);
     CCM_LAUNCHED();
+  }
+  // k_schur_mma's schedule: per row its upper blocks by decreasing list length (ties by block number), cut into tasks of at most
+  // SCHUR_TASK blocks of similar size
+  {
+    std::vector<int> sched((size_t)std::max(nub, 1)), tptr(1, 0);
+    for (int a = 0; a < Kf; a++) {
+      const int ub = h_udiag[a], n = (a + 1 < Kf ? h_udiag[a + 1] : nub) - ub;
+      int* r = sched.data() + ub;
+      std::iota(r, r + n, ub);
+      std::sort(r, r + n, [&](int x, int y) {
+        const unsigned nx = h_pp[x + 1] - h_pp[x], ny = h_pp[y + 1] - h_pp[y];
+        return nx != ny ? nx > ny : x < y;
+      });
+      const int parts = (n + SCHUR_TASK - 1) / SCHUR_TASK;
+      for (int k = 1; k <= parts; k++) tptr.push_back(ub + (int)((long long)n * k / parts));
+    }
+    h->ntasks = (int)tptr.size() - 1;
+    upload_vec(h->u_sched, sched, s);
+    upload_vec(h->task_ptr, tptr, s);
+    h->next_task.alloc(1);
+    int per_sm = 0;
+    CCM_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, (const void*)k_schur_mma, SCHUR_CTA, 0));
+    CCM_REQUIRE(per_sm >= 1, "k_schur_mma does not fit on an SM");
+    h->schur_grid = std::max(1, std::min(h->ntasks, sm_count()));
+    CCM_CUDA(cudaStreamSynchronize(s));   // the host vectors die at the end of this scope
   }
   lap("product lists");
   // ---- measurements: wait for their copy (one-rank path), validate the weights there, apply the edge flags
@@ -1347,6 +1395,34 @@ extern "C" int ccm_ba_debug_coarse(ccm_ba_handle* h, double* Ac, double* Ainv) {
     double st[4];
     CCM_CUDA(cudaMemcpy(st, h->pcg_status.p, sizeof(st), cudaMemcpyDeviceToHost));
     CCM_REQUIRE(st[3] > 0.0, "the coarse matrix has a non-positive pivot");
+  });
+}
+
+extern "C" int ccm_ba_debug_products(ccm_ba_handle* h, int32_t* blk, uint32_t* ptr, int32_t* pairs) {
+  return guarded([&] {
+    CCM_REQUIRE(h, "null handle");
+    CCM_REQUIRE(h->nranks == 1, "debug entry points are single-rank");
+    CCM_CUDA(cudaSetDevice(h->device));
+    cudaStream_t s = h->stream;
+    const int nub = h->nub;
+    std::vector<int> ur((size_t)std::max(nub, 1)), uc((size_t)std::max(nub, 1));
+    std::vector<unsigned> pp((size_t)nub + 1, 0);
+    std::vector<uint2> pr((size_t)std::max<long long>(h->nprod, 1));
+    if (nub) {
+      h->u_row.download(ur.data(), nub, s); h->u_col.download(uc.data(), nub, s); h->u_prod_ptr.download(pp.data(), (size_t)nub + 1, s);
+    }
+    if (h->nprod) h->prod.download(pr.data(), (size_t)h->nprod, s);
+    CCM_CUDA(cudaStreamSynchronize(s));
+    for (int u = 0; u < nub; u++) {
+      if (blk) { blk[2 * (size_t)u] = h->h_slot_pose[ur[u]]; blk[2 * (size_t)u + 1] = h->h_slot_pose[uc[u]]; }
+      if (ptr) ptr[u] = pp[u];
+    }
+    if (ptr) ptr[nub] = pp[nub];
+    if (pairs)
+      for (long long q = 0; q < h->nprod; q++) {
+        pairs[2 * q] = (int32_t)(h->E0 + pr[q].x);
+        pairs[2 * q + 1] = (int32_t)(h->E0 + pr[q].y);
+      }
   });
 }
 

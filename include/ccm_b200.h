@@ -180,6 +180,12 @@ int ccm_ba_debug_step(ccm_ba_handle* h, int robust, double huber_delta, double l
  * nnzb = ccm_ba_info.s_blocks_full.  Any output may be NULL. */
 int ccm_ba_debug_schur_blocks(ccm_ba_handle* h, int32_t* rowptr /*K+1*/, int32_t* col /*nnzb*/, double* val /*nnzb*36*/,
                               double* bschur /*6K*/);
+/* the Schur product lists of the handle: upper block u = (blk[2u], blk[2u+1]) in the caller's pose indices (row <= column, row-major,
+ * columns ascending), its products pairs[2p], pairs[2p+1] for p in [ptr[u], ptr[u+1]): observation pairs (e, o) with e seen by the
+ * row's pose and o by the column's, as positions in the landmark-sorted observation order (the caller's order when obs_mp is
+ * sorted; a stable sort by obs_mp otherwise).  nub = ccm_ba_info.s_blocks_upper, nprod = ccm_ba_info.schur_products.  Any output
+ * may be NULL. */
+int ccm_ba_debug_products(ccm_ba_handle* h, int32_t* blk /*2*nub*/, uint32_t* ptr /*nub+1*/, int32_t* pairs /*2*nprod*/);
 /* the PCG path the handle runs: out[0] implementation (1 k_pcg, 2 k_pcg2), out[1] k_pcg CTA size, out[2] coarse aggregate size,
  * out[3] coarse nodes (0: no coarse space) */
 int ccm_ba_debug_paths(ccm_ba_handle* h, int32_t* out /*4*/);
