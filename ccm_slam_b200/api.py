@@ -289,6 +289,16 @@ class BAHandle:
         _chk(lib().ccm_ba_debug_products(self._h, _p(blk), _p(ptr), _p(pairs)))
         return dict(blk=blk[:nub], ptr=ptr.astype(np.int64), pairs=pairs[:nprod])
 
+    def debug_schedule(self):
+        """the Schur kernel's schedule (ccm_ba_debug_schedule): ntasks, grid (CTAs of its launch), task_ptr (ntasks+1,) ranges in
+        sched (nub,), the upper block numbers of debug_products"""
+        counts = np.zeros(2, np.int32)
+        _chk(lib().ccm_ba_debug_schedule(self._h, _p(counts), None, None))
+        nt, nub = int(counts[0]), self.info()["s_blocks_upper"]
+        tp = np.empty(nt + 1, np.int32); sched = np.empty(max(nub, 1), np.int32)
+        _chk(lib().ccm_ba_debug_schedule(self._h, None, _p(tp), _p(sched)))
+        return dict(ntasks=nt, grid=int(counts[1]), task_ptr=tp, sched=sched[:nub])
+
     PATH_KEYS = ("pcg_impl", "pcg_block", "pcg_agg", "pcg_nc")
 
     def debug_paths(self):

@@ -1426,6 +1426,18 @@ extern "C" int ccm_ba_debug_products(ccm_ba_handle* h, int32_t* blk, uint32_t* p
   });
 }
 
+extern "C" int ccm_ba_debug_schedule(ccm_ba_handle* h, int32_t* counts, int32_t* task_ptr, int32_t* sched) {
+  return guarded([&] {
+    CCM_REQUIRE(h, "null handle");
+    CCM_CUDA(cudaSetDevice(h->device));
+    cudaStream_t s = h->stream;
+    if (counts) { counts[0] = h->ntasks; counts[1] = h->schur_grid; }
+    if (task_ptr) h->task_ptr.download(task_ptr, (size_t)h->ntasks + 1, s);
+    if (sched && h->nub) h->u_sched.download(sched, (size_t)h->nub, s);
+    CCM_CUDA(cudaStreamSynchronize(s));
+  });
+}
+
 extern "C" int ccm_ba_debug_paths(ccm_ba_handle* h, int32_t* out) {
   return guarded([&] {
     CCM_REQUIRE(h && out, "null argument");

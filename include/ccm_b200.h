@@ -186,6 +186,10 @@ int ccm_ba_debug_schur_blocks(ccm_ba_handle* h, int32_t* rowptr /*K+1*/, int32_t
  * sorted; a stable sort by obs_mp otherwise).  nub = ccm_ba_info.s_blocks_upper, nprod = ccm_ba_info.schur_products.  Any output
  * may be NULL. */
 int ccm_ba_debug_products(ccm_ba_handle* h, int32_t* blk /*2*nub*/, uint32_t* ptr /*nub+1*/, int32_t* pairs /*2*nprod*/);
+/* the Schur kernel's schedule: counts[0] tasks, counts[1] CTAs of its launch; task t covers sched[task_ptr[t] .. task_ptr[t+1]),
+ * upper block numbers as in ccm_ba_debug_products.  Call with task_ptr and sched NULL to learn the number of tasks first.  Any
+ * output may be NULL. */
+int ccm_ba_debug_schedule(ccm_ba_handle* h, int32_t* counts /*2*/, int32_t* task_ptr /*ntasks+1*/, int32_t* sched /*nub*/);
 /* the PCG path the handle runs: out[0] implementation (1 k_pcg, 2 k_pcg2), out[1] k_pcg CTA size, out[2] coarse aggregate size,
  * out[3] coarse nodes (0: no coarse space) */
 int ccm_ba_debug_paths(ccm_ba_handle* h, int32_t* out /*4*/);
