@@ -26,7 +26,7 @@ def needs_build() -> bool:
     if not os.path.exists(OUT):
         return True
     t = os.path.getmtime(OUT)
-    deps = sources() + glob.glob(os.path.join(CSRC, "*.cuh")) + glob.glob(os.path.join(HERE, "..", "include", "*.h")) + [__file__]
+    deps = sources() + glob.glob(os.path.join(CSRC, "*.cuh")) + glob.glob(os.path.join(CSRC, "*.h")) + glob.glob(os.path.join(HERE, "..", "include", "*.h")) + [__file__]
     return any(os.path.getmtime(d) > t for d in deps)
 
 

@@ -2,14 +2,13 @@
 //
 // Control flow restates g2o's OptimizationAlgorithmLevenberg::solve + SparseOptimizer::optimize
 // (G/core/optimization_algorithm_levenberg.cpp:61-164, G/core/sparse_optimizer.cpp:354-419): the scalar LM schedule
-// (lambda, nu, rho, stop rules, force-stop flag polling) runs on the host, every O(E)/O(P)/O(K) step is a kernel from
+// (lm_schedule.h; force-stop flag polling here) runs on the host, every O(E)/O(P)/O(K) step is a kernel from
 // ba_kernels.cuh on the handle's stream.  push/pop/discardTop become a (current, trial) double buffer.
 // Multi-GPU: landmarks (and their observations) are sharded across ranks; per LM iteration one all-reduce of
 // [Hpp | bp | chi2], per LM trial one all-reduce of [S upper blocks | bschur part] and one of [chi2, scale].
 #include <algorithm>
 #include <chrono>
 #include <cmath>
-#include <limits>
 #include <numeric>
 
 #include <cub/device/device_radix_sort.cuh>
@@ -17,6 +16,7 @@
 
 #include "ba_kernels.cuh"
 #include "common.cuh"
+#include "lm_schedule.h"
 #include "pcg2.cuh"
 
 namespace ccm {
@@ -54,7 +54,6 @@ struct ccm_ba_handle {
   std::vector<uint8_t> h_flags;     // local shard, sorted order
   std::vector<int> h_pose_slot, h_slot_pose;
   int words = 0, nub = 0;
-  void* pcg_fn = nullptr;  // k_pcg variant matching pcg_block
   long long nnzb = 0, nprod = 0;
   // state
   DevBuf<double> pose0, poseA, poseB, intr, pt0, ptA, ptB;
@@ -73,7 +72,7 @@ struct ccm_ba_handle {
   int nunits = 0, lin_grid = 1, bs_grid = 1;
   DevBuf<double> Hbuf;                    // [Hpp Kf*36 | bp Kf*6 | chi2_cur | maxdiag-bits]
   DevBuf<double> Ubuf;                    // [U_val nub*36 | bneg Kf*6]
-  DevBuf<double> s_val, Minv, bschur;
+  DevBuf<double> s_val, Minv, bschur, dxl;
   DevBuf<int> s_rowptr, s_col, s_row, s_diag, csr_u, u_row, u_col, u_diag, word_prefix;
   DevBuf<unsigned> bitmap, u_prod_ptr;
   DevBuf<uint2> prod;
@@ -82,13 +81,11 @@ struct ccm_ba_handle {
   DevBuf<float4> kobs;            // per free pose: (u, v, signed w, landmark) of its observations, packed
   DevBuf<unsigned> kobs_ptr;
   // pcg
-  DevBuf<double> x, pr, pz, pp, pq, pcg_partials, pcg_status, dxl, pcg_Ac, pcg_rc, pcg_yc;
-  int pcg_agg = 0, pcg_nc = 0, pcg_refresh = 4, pcg_age = 0, pcg_prolong = 0;
+  PcgDriver<6> pcg;               // k_pcg, and the x / r / p / q / partials / bar / status k_pcg2 reads as well
+  int pcg_refresh = 4, pcg_age = 0, pcg_last_mode = 1;
   bool pcg_coarse_valid = false;  // Ac holds a usable inverse from an earlier trial
-  DevBuf<unsigned> pcg_bar;
   DevBuf<long long> pcg_prof;  // allocated only with CCM_PCG_PROF=1
   DevBuf<int> jac_fail;
-  int pcg_grid = 0, pcg_block = 256, pcg_last_mode = 1;
   // second-generation PCG (pcg2.cuh): TMA-streamed product, three synchronisations per iteration, rows distributed over the ranks
   struct Pcg2 {
     bool on = false;
@@ -182,7 +179,7 @@ void launch_linearize(ccm_ba_handle* h, int robust, double delta, int mode, doub
 
 void launch_backsub(ccm_ba_handle* h, double lambda, double* dx_points) {
   k_backsub_points<<<h->bs_grid, LIN_TILE, 0, h->stream>>>(h->units.p, h->nunits, h->lm_ptr.p, h->o_kf.p, h->pose_slot.p, h->Z.p,
-                                                           h->Hll(), h->bl(), h->x.p, h->pt_cur, h->Pl, lambda, h->pt_trial, dx_points,
+                                                           h->Hll(), h->bl(), h->pcg.x.p, h->pt_cur, h->Pl, lambda, h->pt_trial, dx_points,
                                                            h->partials.p);
   CCM_LAUNCHED();
 }
@@ -275,40 +272,23 @@ void step_finalize(ccm_ba_handle* h, double lambda) {
   CCM_LAUNCHED();
 }
 
-PcgArgs pcg_args(ccm_ba_handle* h, double tol, int max_iter) {
-  PcgArgs a;
-  a.n = h->Kf; a.rowptr = h->s_rowptr.p; a.col = h->s_col.p; a.val = h->s_val.p; a.Minv = h->Minv.p; a.b = h->bschur.p;
-  a.x = h->x.p; a.r = h->pr.p; a.z = h->pz.p; a.p = h->pp.p; a.q = h->pq.p;
-  a.partials = h->pcg_partials.p; a.bar = h->pcg_bar.p; a.tol = tol; a.max_iter = max_iter; a.status = h->pcg_status.p;
-  a.agg = h->pcg_agg; a.nc = h->pcg_nc; a.Ac = h->pcg_Ac.p; a.rc = h->pcg_rc.p; a.yc = h->pcg_yc.p;
-  a.prof = h->pcg_prof.p;
-  a.prolong = h->pcg_prolong;
-  return a;
-}
-
 void step_pcg(ccm_ba_handle* h, double tol, int max_iter) {
   cudaStream_t s = h->stream;
   KernelSpan sp(h, CCM_BA_K_PCG);
-  CCM_CUDA(cudaMemsetAsync(h->pcg_bar.p, 0, 2 * sizeof(unsigned), s));
-  PcgArgs a = pcg_args(h, tol, max_iter);
-  a.coarse_mode = (h->pcg_coarse_valid && h->pcg_age < h->pcg_refresh) ? 2 : 1;
-  h->pcg_last_mode = a.coarse_mode;
+  PcgDriver<6>& pcg = h->pcg;
+  const int coarse_mode = (h->pcg_coarse_valid && h->pcg_age < h->pcg_refresh) ? 2 : 1;
+  h->pcg_last_mode = coarse_mode;
   if (h->p2.on) {
     ccm_ba_handle::Pcg2& d = h->p2;
-    if (a.coarse_mode == 1 && a.agg > 0) {  // (re)build the coarse inverse with k_pcg's set-up phase: no iteration
-      PcgArgs setup = a;
-      setup.max_iter = 0;
-      void* sargs[] = {&setup};
-      CCM_CUDA(cudaLaunchCooperativeKernel(h->pcg_fn, dim3(h->pcg_grid), dim3(h->pcg_block), sargs, 0, s));
-      CCM_LAUNCHED();
-    }
-    const int nC = a.agg > 0 ? 6 * a.nc : 0;
+    // (re)build the coarse inverse with k_pcg's set-up phase: no iteration
+    if (coarse_mode == 1 && pcg.agg > 0) pcg.launch(tol, 0, coarse_mode, h->pcg_prof.p, s);
+    const int nC = pcg.nC();
     Pcg2Args b;
     b.n = h->Kf; b.val = h->s_val.p; b.items = d.items.p; b.cta_row = d.cta_row.p; b.cta_item = d.cta_item.p;
-    b.Minv = h->Minv.p; b.b = h->bschur.p; b.x = h->x.p; b.r = h->pr.p; b.q = h->pq.p; b.p = h->pp.p;
-    b.partials = h->pcg_partials.p; b.bar = h->pcg_bar.p; b.tol = tol; b.max_iter = max_iter; b.status = h->pcg_status.p;
-    b.agg = a.agg; b.nc = a.nc; b.prolong = a.prolong;
-    b.Ainv = nC > 0 ? coarse_inverse(h->pcg_Ac.p, nC) : nullptr;
+    b.Minv = h->Minv.p; b.b = h->bschur.p; b.x = pcg.x.p; b.r = pcg.r.p; b.q = pcg.q.p; b.p = pcg.p.p;
+    b.partials = pcg.partials.p; b.bar = pcg.bar.p; b.tol = tol; b.max_iter = max_iter; b.status = pcg.status.p;
+    b.agg = pcg.agg; b.nc = pcg.nc; b.prolong = pcg.prolong;
+    b.Ainv = nC > 0 ? coarse_inverse(pcg.Ac.p, nC) : nullptr;
     b.yc = d.yc.p; b.tpart = d.tpart.p;
     b.rank = h->rank; b.nranks = h->nranks; b.r0 = d.r0; b.r1 = d.r1; b.win = d.d_win.p;
     b.off_z = d.lay.off_z; b.off_x = d.lay.off_x;
@@ -318,7 +298,7 @@ void step_pcg(ccm_ba_handle* h, double tol, int max_iter) {
     b.ll_epoch0 = (unsigned)((d.launches & 0x7FFFFu) << 13) | 0x1000u;   // + 2 (it + 1) + {0, 1} <= 4003 below bit 12; never 0
     b.timeout_cycles = d.timeout_cycles;
     b.prof = h->pcg_prof.p;
-    CCM_CUDA(cudaMemsetAsync(h->pcg_bar.p, 0, 2 * sizeof(unsigned), s));
+    CCM_CUDA(cudaMemsetAsync(pcg.bar.p, 0, 2 * sizeof(unsigned), s));
     CCM_CUDA(cudaMemsetAsync(d.tpart.p, 0, d.tpart.bytes(), s));
     CCM_CUDA(cudaMemsetAsync(d.window + d.lay.off_ctl, 0, sizeof(unsigned), s));
     void* bargs[] = {&b};
@@ -326,9 +306,7 @@ void step_pcg(ccm_ba_handle* h, double tol, int max_iter) {
     CCM_LAUNCHED();
     return;
   }
-  void* args[] = {&a};
-  CCM_CUDA(cudaLaunchCooperativeKernel(h->pcg_fn, dim3(h->pcg_grid), dim3(h->pcg_block), args, 0, s));
-  CCM_LAUNCHED();
+  pcg.launch(tol, max_iter, coarse_mode, h->pcg_prof.p, s);
 }
 
 // pcg2.cuh set-up: own rows, item records, CTA cuts, exchange window (IPC-mapped on every rank when nranks > 1).
@@ -340,13 +318,13 @@ void setup_pcg2(ccm_ba_handle* h, const std::vector<int>& rowptr) {
   const int impl = env_int("CCM_PCG_IMPL", 0);
   if (impl == 1 || h->Kf < 1 || h->Kf < h->nranks) return;
   if (impl != 2 && rowptr[h->Kf] < env_int("CCM_PCG2_MIN_BLOCKS", 200000)) return;
-  if (h->pcg_agg > 0 && 6 * h->pcg_nc > P2_MAX_NC) return;
+  const int nC = h->pcg.nC();
+  if (nC > P2_MAX_NC) return;
   static_assert(sizeof(cudaIpcMemHandle_t) == 64, "IPC handle size");
   ccm_ba_handle::Pcg2& d = h->p2;
   cudaStream_t s = h->stream;
   const int N = h->nranks, Kf = h->Kf;
   d.rank = h->rank;
-  const int nC = h->pcg_agg > 0 ? 6 * h->pcg_nc : 0;
   // contiguous block rows per rank, cut where the block-count prefix crosses k * nnzb / N
   auto cut = [&](int k) {
     if (k <= 0) return 0;
@@ -397,8 +375,7 @@ void setup_pcg2(ccm_ba_handle* h, const std::vector<int>& rowptr) {
   }
   d.yc.alloc_zero(std::max<size_t>((size_t)2 * nC, 1), s);
   d.tpart.alloc_zero(std::max<size_t>((size_t)2 * nC, 1), s);
-  if ((size_t)3 * d.grid > h->pcg_partials.n) h->pcg_partials.alloc((size_t)3 * d.grid);
-  if (h->pcg_bar.n < 2) h->pcg_bar.alloc_zero(2, s);
+  if ((size_t)3 * d.grid > h->pcg.partials.n) h->pcg.partials.alloc((size_t)3 * d.grid);
   // exchange window
   d.lay = pcg2_layout(Kf, N, nC);
   if (N == 1) {   // no peer maps it: stream-ordered pool memory (cudaMalloc / cudaFree synchronise the device on every create / destroy)
@@ -449,7 +426,7 @@ void step_update_and_residual(ccm_ba_handle* h, double lambda, int robust, doubl
   cudaStream_t s = h->stream;
   const int g1 = grid_stride(h->K);
   size_t ev0 = h->profile ? ev_record(h) : 0;
-  k_update_poses<<<g1, TPB, 0, s>>>(h->pose_cur, h->pose_slot.p, h->x.p, h->bp(), h->K, lambda, h->pose_trial, h->partials.p);
+  k_update_poses<<<g1, TPB, 0, s>>>(h->pose_cur, h->pose_slot.p, h->pcg.x.p, h->bp(), h->K, lambda, h->pose_trial, h->partials.p);
   CCM_LAUNCHED();
   sum_partials_to(h, g1, h->scal.p + 2);
   launch_backsub(h, lambda, dx_points);
@@ -872,32 +849,20 @@ void build(ccm_ba_handle* h, const ccm_ba_problem* p) {
   h->Ubuf.alloc_zero((size_t)nub * 36 + (size_t)Kf * 6 + 1, s);
   h->s_val.alloc(std::max<long long>(nnzb * 36, 1)); h->Minv.alloc(std::max((size_t)Kf * 36, (size_t)1));
   h->bschur.alloc(std::max((size_t)Kf * 6, (size_t)1));
-  const size_t nv = std::max((size_t)Kf * 6, (size_t)1);
-  h->x.alloc_zero(nv, s); h->pr.alloc(nv); h->pz.alloc(nv); h->pp.alloc(2 * nv); h->pq.alloc(nv);
-  h->dxl.alloc(std::max((size_t)Pl * 3, (size_t)1));
-  h->pcg_status.alloc_zero(4, s); h->pcg_bar.alloc_zero(2, s); h->jac_fail.alloc_zero(1, s);
-  // one warp per block row: one fat CTA per SM (cheap grid barrier) when the rows fill the chip, otherwise 256-thread CTAs
-  // (two per SM) so that a small system still spreads over many SMs.  512x1 and 256x2 leave the product loop 128 registers.
-  h->pcg_block = ((long long)Kf * 32 >= (long long)sm_count() * PCG_TPB) ? env_int("CCM_PCG_BLOCK", 512) : 256;
-  CCM_REQUIRE(h->pcg_block == 256 || h->pcg_block == 512 || h->pcg_block == 1024, "CCM_PCG_BLOCK must be 256, 512 or 1024");
-  h->pcg_fn = h->pcg_block == 1024 ? (void*)k_pcg<6, 1024, 1> : h->pcg_block == 512 ? (void*)k_pcg<6, 512, 1> : (void*)k_pcg<6, 256, 2>;
-  int per_sm = 0;
-  CCM_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, (const void*)h->pcg_fn, h->pcg_block, 0));
-  CCM_REQUIRE(per_sm >= 1, "k_pcg does not fit on an SM");
-  per_sm = std::min(per_sm, h->pcg_block == 256 ? 2 : 1);
-  h->pcg_grid = std::max(1, std::min(sm_count() * per_sm, div_up((long long)std::max(Kf, 1) * 32, h->pcg_block)));
-  h->pcg_partials.alloc((size_t)3 * h->pcg_grid);
-  if (env_int("CCM_PCG_PROF", 0)) h->pcg_prof.alloc_zero(8, s);
   // coarse space: <= 128 aggregates for small systems, <= 384 for long trajectories where the smooth modes dominate the
   // iteration count; the inverse is refreshed every 2nd solve (measured sweeps: tools/ba_probe.py with CCM_PCG_NC/REFRESH)
   // CCM_PCG_PROLONG=1: piecewise-linear prolongation (pcg.cuh); half the coarse nodes then already beat the constant P
-  h->pcg_prolong = env_int("CCM_PCG_PROLONG", 1) ? 1 : 0;  // cfg5: 1538 -> 617 PCG iterations per Global BA at 192 coarse nodes
+  const int prolong = env_int("CCM_PCG_PROLONG", 1) ? 1 : 0;  // cfg5: 1538 -> 617 PCG iterations per Global BA at 192 coarse nodes
   // PCG iterations per Global BA on cfg5: NC 192 refresh 4: 617, NC 192 refresh 2: 545, NC 256 refresh 2: 400, NC 256 refresh 1: 384,
   // NC 384 refresh 4: 357 (its 2304^2 inverse is the most expensive), NC 128 refresh 1: 1014; refresh 8 (one inverse per BA): 1950
   // From Kf >= 8192 (cfg5: Kf = 9999) 320 nodes: an iteration of k_pcg2 there costs about 110 us, so the iterations a larger coarse
   // space saves outweigh its dearer inverse; below that the iterations are cheaper and 256 nodes stay the better trade.
-  pcg_coarse_shape(Kf, env_int("CCM_PCG_NC", Kf >= 4096 ? (h->pcg_prolong ? (Kf >= 8192 ? 320 : 256) : 384) : 128), &h->pcg_agg,
-                   &h->pcg_nc);
+  h->pcg.shape(Kf, env_int("CCM_PCG_NC", Kf >= 4096 ? (prolong ? (Kf >= 8192 ? 320 : 256) : 384) : 128), prolong);
+  // the PCG's vectors follow the system's directly: allocated after dxl, the same code ran cfg5 1.2 % slower (H100 80GB HBM3, 700 W)
+  h->pcg.alloc({h->s_rowptr.p, h->s_col.p, h->s_val.p, h->Minv.p, h->bschur.p}, s);
+  h->dxl.alloc(std::max((size_t)Pl * 3, (size_t)1));
+  h->jac_fail.alloc_zero(1, s);
+  if (env_int("CCM_PCG_PROF", 0)) h->pcg_prof.alloc_zero(8, s);
   // refresh 1 / 2 / 4 with NC 256: 384 / 400 / 496 iterations per cfg5 Global BA.  An iteration of k_pcg2 costs about 120 us and
   // the set-up launch that rebuilds the 1536^2 inverse 2.0 ms, so one BA takes 173 / 167 / 174 ms; cfg4 (k_pcg, nC = 690) takes
   // 27.3 / 24.5 ms at refresh 1 / 2 (H100 80GB HBM3, 700 W).  Every size rebuilds every 2nd solve.
@@ -905,10 +870,6 @@ void build(ccm_ba_handle* h, const ccm_ba_problem* p) {
   //   256 / 2: 400, 167.5   320 / 2: 262, 157.1   384 / 2: 212, 160.3
   //   256 / 1: 384, 172.9   320 / 1: 246, 168.7   384 / 1: 197, 179.9
   h->pcg_refresh = std::max(1, env_int("CCM_PCG_REFRESH", 2));
-  {
-    const size_t nC = (size_t)6 * h->pcg_nc;
-    h->pcg_Ac.alloc(std::max(2 * nC * nC, (size_t)1)); h->pcg_rc.alloc(std::max(2 * nC, (size_t)1)); h->pcg_yc.alloc(std::max(nC, (size_t)1));
-  }
   setup_pcg2(h, h_rowptr);
   h->partials.alloc((size_t)std::max({sm_count() * 8 + 8, h->lin_grid, h->bs_grid}));
   h->scal.alloc_zero(16, s);
@@ -1007,89 +968,54 @@ void optimize(ccm_ba_handle* h, const ccm_ba_options* o, ccm_ba_result* r) {
     // g2o: landmarks-only graphs are still optimised, but every cslam call site has free poses; keep it simple
     ret_iters = h->E == 0 ? -1 : 0;
   }
-  double lambda = -1, ni = 2;
-  int nBad = 0;
-  bool ok = true;
-  for (int it = 0; h->Kf > 0 && h->E > 0 && it < o->iterations && !terminate() && ok; it++) {
+  LmSchedule lm{max_trials};
+  for (int it = 0; h->Kf > 0 && h->E > 0 && it < o->iterations && !terminate(); it++) {
     // from the second iteration on lambda is known before the linearisation, which then forms Z as well; the first iteration takes
     // lambda from the diagonal it has just built and forms Z in a second, Z-only pass
-    step_linearize(h, robust, delta, it == 0 ? 0 : LIN_Z, lambda);
-    double currentChi;
+    step_linearize(h, robust, delta, it == 0 ? 0 : LIN_Z, lm.lambda);
     if (it == 0) {
       const double maxdiag = step_max_diag(h);
       if (!(maxdiag > 0.0)) {  // every edge is inactive (weight 0): nothing to optimise, the estimate is left alone
         ret_iters = -1;
         break;
       }
-      currentChi = h->h_scal[8];
-      lambda = o->lambda_init > 0 ? o->lambda_init : 1e-5 * maxdiag;
-      ni = 2; nBad = 0;
-      r->chi2_initial = currentChi;
-      step_z(h, robust, delta, lambda);
+      lm.start(o->lambda_init, maxdiag);
+      lm.begin_iteration(h->h_scal[8]);
+      r->chi2_initial = lm.currentChi;
+      step_z(h, robust, delta, lm.lambda);
     } else {
-      currentChi = read_chi2_cur(h);
+      lm.begin_iteration(read_chi2_cur(h));
     }
-    const double iniChi = currentChi;
-    double tempChi = currentChi, rho = 0, lambda_used = lambda;
-    int qmax = 0, last_pcg_it = 0;
-    double last_relres = 0;
     do {
-      lambda_used = lambda;
-      if (qmax > 0) step_z(h, robust, delta, lambda);   // the trial before was rejected: same estimate, larger lambda
+      if (lm.qmax > 0) step_z(h, robust, delta, lm.lambda);   // the trial before was rejected: same estimate, larger lambda
       step_schur(h);
-      step_finalize(h, lambda);
+      step_finalize(h, lm.lambda);
       step_pcg(h, pcg_tol, pcg_max);
-      step_update_and_residual(h, lambda, robust, delta, nullptr, stop_local());
+      step_update_and_residual(h, lm.lambda, robust, delta, nullptr, stop_local());
       CCM_CUDA(cudaMemcpyAsync(h->h_scal, h->scal.p, 3 * sizeof(double), cudaMemcpyDeviceToHost, s));
       if (h->nranks > 1) CCM_CUDA(cudaMemcpyAsync(h->h_scal + 13, h->scal.p + 3, sizeof(double), cudaMemcpyDeviceToHost, s));
-      CCM_CUDA(cudaMemcpyAsync(h->h_scal + 3, h->pcg_status.p, 4 * sizeof(double), cudaMemcpyDeviceToHost, s));
+      CCM_CUDA(cudaMemcpyAsync(h->h_scal + 3, h->pcg.status.p, 4 * sizeof(double), cudaMemcpyDeviceToHost, s));
       CCM_CUDA(cudaMemcpyAsync(h->h_scal + 7, h->jac_fail.p, sizeof(int), cudaMemcpyDeviceToHost, s));
       CCM_CUDA(cudaStreamSynchronize(s));
       if (h->profile) collect_spans(h);
-      tempChi = h->h_scal[0];
       if (h->nranks > 1) stop_all = h->h_scal[13] > 0.0;
       const int pcg_it = (int)h->h_scal[3];
       const int pcg_flag = (int)h->h_scal[5];
       int jfail;
       memcpy(&jfail, h->h_scal + 7, sizeof(int));
       if (h->pcg_last_mode == 1) { h->pcg_coarse_valid = h->h_scal[6] > 0; h->pcg_age = 1; } else h->pcg_age++;
-      last_pcg_it = pcg_it; last_relres = h->h_scal[4];
       r->pcg_iters_total += pcg_it;
       if (pcg_flag == 1) r->pcg_not_converged++;
       if (pcg_flag == 3) throw Error(CCM_ERR_NCCL, "distributed PCG: a peer's packet did not arrive within CCM_PCG_DIST_TIMEOUT_MS");
-      const bool ok2 = !(pcg_flag == 2 || jfail);  // linear solve failed (not SPD): the trial is rejected
-      if (!ok2) tempChi = std::numeric_limits<double>::max();
-      rho = currentChi - tempChi;
-      double scale = h->h_scal[1] + h->h_scal[2];
-      scale += 1e-3;
-      rho /= scale;
-      if (rho > 0 && std::isfinite(tempChi)) {
-        double alpha = 1. - std::pow((2 * rho - 1), 3);
-        alpha = std::min(alpha, 2. / 3.);
-        const double scaleFactor = std::max(1. / 3., alpha);
-        lambda *= scaleFactor;
-        ni = 2;
-        currentChi = tempChi;
+      const bool solved = !(pcg_flag == 2 || jfail);  // linear solve failed (not SPD): the trial is rejected
+      if (lm.trial(h->h_scal[0], h->h_scal[1] + h->h_scal[2], solved, pcg_it, h->h_scal[4])) {  // rejected: pop, the estimate stays
         std::swap(h->pose_cur, h->pose_trial);  // discardTop: the trial state becomes the estimate
         std::swap(h->pt_cur, h->pt_trial);
-      } else {
-        lambda *= ni;
-        ni *= 2;  // pop: the estimate stays
       }
-      qmax++;
       r->trials_total++;
-    } while (rho < 0 && qmax < max_trials && !terminate());
+    } while (lm.retry() && !terminate());
     ret_iters++;
-    if (r->trace && r->trace_len < r->trace_cap) {
-      double* tr = r->trace + (size_t)r->trace_len * CCM_TRACE_COLS;
-      tr[0] = it; tr[1] = lambda_used; tr[2] = currentChi; tr[3] = rho; tr[4] = qmax; tr[5] = lambda;
-      tr[6] = last_pcg_it; tr[7] = last_relres;
-      r->trace_len++;
-    }
-    r->chi2_final = currentChi; r->lambda_final = lambda;
-    if (qmax == max_trials || rho == 0) { ok = false; continue; }
-    if ((iniChi - currentChi) * 1e3 < iniChi) nBad++; else nBad = 0;
-    if (nBad >= 3) { ok = false; continue; }
+    if (lm.end_iteration(r, it)) break;
   }
   r->iters_done = ret_iters;
   CCM_CUDA(cudaEventRecord(evB, s));
@@ -1277,8 +1203,8 @@ extern "C" int ccm_ba_debug_schur(ccm_ba_handle* h, int robust, double huber_del
     step_update_and_residual(h, lambda, robust, huber_delta, h->dxl.p);
     const int K = h->K, Kf = h->Kf, Pl = h->Pl;
     std::vector<double> hx((size_t)Kf * 6), hdl((size_t)Pl * 3), hb((size_t)Kf * 6), st(3);
-    h->x.download(hx.data(), hx.size(), s); h->dxl.download(hdl.data(), hdl.size(), s);
-    h->bschur.download(hb.data(), hb.size(), s); h->pcg_status.download(st.data(), 3, s);
+    h->pcg.x.download(hx.data(), hx.size(), s); h->dxl.download(hdl.data(), hdl.size(), s);
+    h->bschur.download(hb.data(), hb.size(), s); h->pcg.status.download(st.data(), 3, s);
     CCM_CUDA(cudaStreamSynchronize(s));
     if (pcg_iters) *pcg_iters = (int)st[0];
     if (pcg_relres) *pcg_relres = st[1];
@@ -1320,7 +1246,7 @@ extern "C" int ccm_ba_debug_step(ccm_ba_handle* h, int robust, double huber_delt
     std::vector<double> hx((size_t)std::max(Kf, 1) * 6, 0.0);
     for (int a = 0; a < Kf; a++) memcpy(hx.data() + (size_t)a * 6, dx_pose + 6 * (size_t)h->h_slot_pose[a], 6 * sizeof(double));
     step_linearize(h, robust, huber_delta, LIN_Z, lambda);
-    if (Kf > 0) h->x.upload(hx.data(), (size_t)Kf * 6, s);
+    if (Kf > 0) h->pcg.x.upload(hx.data(), (size_t)Kf * 6, s);
     step_update_and_residual(h, lambda, robust, huber_delta, h->dxl.p);
     std::vector<double> hp((size_t)K * 7), hq((size_t)Pl * 3), hd((size_t)Pl * 3), sc(3);
     if (K > 0) CCM_CUDA(cudaMemcpyAsync(hp.data(), h->pose_trial, hp.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
@@ -1377,23 +1303,18 @@ extern "C" int ccm_ba_debug_schur_blocks(ccm_ba_handle* h, int32_t* rowptr, int3
 extern "C" int ccm_ba_debug_coarse(ccm_ba_handle* h, double* Ac, double* Ainv) {
   return guarded([&] {
     CCM_REQUIRE(h && Ac && Ainv, "null argument");
-    CCM_REQUIRE(h->pcg_agg > 0 && h->pcg_nc > 0, "the handle has no coarse space");
+    const int nC = h->pcg.nC();
+    CCM_REQUIRE(nC > 0, "the handle has no coarse space");
     cudaStream_t s = h->stream;
-    const int nC = 6 * h->pcg_nc;
     const size_t bytes = (size_t)nC * nC * sizeof(double);
-    PcgArgs a = pcg_args(h, 0.0, 0);
     for (int mode : {3, 1}) {  // the assembled matrix, then the set-up launch step_pcg makes before k_pcg2
-      a.coarse_mode = mode;
-      CCM_CUDA(cudaMemsetAsync(h->pcg_bar.p, 0, 2 * sizeof(unsigned), s));
-      void* args[] = {&a};
-      CCM_CUDA(cudaLaunchCooperativeKernel(h->pcg_fn, dim3(h->pcg_grid), dim3(h->pcg_block), args, 0, s));
-      CCM_LAUNCHED();
-      CCM_CUDA(cudaMemcpyAsync(mode == 3 ? Ac : Ainv, mode == 3 ? h->pcg_Ac.p : coarse_inverse(h->pcg_Ac.p, nC), bytes,
+      h->pcg.launch(0.0, 0, mode, h->pcg_prof.p, s);
+      CCM_CUDA(cudaMemcpyAsync(mode == 3 ? Ac : Ainv, mode == 3 ? h->pcg.Ac.p : coarse_inverse(h->pcg.Ac.p, nC), bytes,
                                cudaMemcpyDeviceToHost, s));
     }
     CCM_CUDA(cudaStreamSynchronize(s));
     double st[4];
-    CCM_CUDA(cudaMemcpy(st, h->pcg_status.p, sizeof(st), cudaMemcpyDeviceToHost));
+    CCM_CUDA(cudaMemcpy(st, h->pcg.status.p, sizeof(st), cudaMemcpyDeviceToHost));
     CCM_REQUIRE(st[3] > 0.0, "the coarse matrix has a non-positive pivot");
   });
 }
@@ -1442,9 +1363,9 @@ extern "C" int ccm_ba_debug_paths(ccm_ba_handle* h, int32_t* out) {
   return guarded([&] {
     CCM_REQUIRE(h && out, "null argument");
     out[0] = h->p2.on ? 2 : 1;
-    out[1] = h->pcg_block;
-    out[2] = h->pcg_agg;
-    out[3] = h->pcg_nc;
+    out[1] = h->pcg.block;
+    out[2] = h->pcg.agg;
+    out[3] = h->pcg.nc;
   });
 }
 

@@ -18,6 +18,8 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include "common.cuh"
+
 namespace ccm {
 
 constexpr int TPB = 256;
@@ -28,7 +30,7 @@ constexpr int GJB = 32;
 constexpr int GJ_CW = 128;     // column chunk a CTA stages per sweep
 constexpr int GJ_LDP = GJB + 4;     // padded row strides of the shared pivot inverse / pivot rows: the B fragments of
 constexpr int GJ_LDR = GJ_CW + 4;   // mma.m8n8k4 read 4 rows x 8 columns, unpadded those 4 rows fall into the same banks
-constexpr int PCG_TPB = 1024;  // one fat CTA per SM keeps the grid barrier at one participant per SM (132 on an H100 SXM)
+constexpr int PCG_TPB = 1024;  // most threads of a CTA (sizes red[]); the rows fill the chip when n * 32 >= SMs * PCG_TPB (PcgDriver)
 
 // The ping-pong buffer of Ac (2 (BS nc)^2 doubles) that holds the coarse inverse after the set-up: the sweep count's parity.
 __host__ __device__ inline double* coarse_inverse(double* Ac, int nC) {
@@ -124,8 +126,8 @@ __device__ __forceinline__ double sum_partials_dev(const double* partials, int g
   return warp_sum(v);
 }
 
-// MAXT/MINB: launch bounds of the variant (1024x1 leaves 64 registers per thread, 512x1 and 256x2 leave 128)
-template <int BS, int MAXT = PCG_TPB, int MINB = 1>
+// MAXT/MINB: launch bounds of the variant (512x1 and 256x2 both leave 128 registers per thread)
+template <int BS, int MAXT, int MINB>
 __global__ void __launch_bounds__(MAXT, MINB) k_pcg(PcgArgs A) {
   constexpr int BB = BS * BS;
   __shared__ double red[PCG_TPB / 32];
@@ -133,7 +135,7 @@ __global__ void __launch_bounds__(MAXT, MINB) k_pcg(PcgArgs A) {
   __shared__ double gj_pi[GJB * GJ_LDP];
   __shared__ double gj_vr[2][GJB], gj_vc[2][GJB];
   __shared__ int gj_bad;
-  const int bdim = blockDim.x;  // 256 (small systems: spread over more SMs) or PCG_TPB
+  const int bdim = blockDim.x;  // 256 (small systems: spread over more SMs) or 512
   const int lane = threadIdx.x & 31;
   const int gw = (blockIdx.x * bdim + threadIdx.x) >> 5;
   const int nw = (gridDim.x * bdim) >> 5;
@@ -551,5 +553,59 @@ inline void pcg_coarse_shape(int n, int nc_max, int* agg, int* nc) {
   if (*agg < 1) *agg = 1;
   *nc = (n + *agg - 1) / *agg;
 }
+
+// The system k_pcg solves: n x n blocks of BS x BS in block-CSR (rowptr, col, val), the inverses of its diagonal blocks, b.
+struct PcgSystem { const int* rowptr; const int* col; const double* val; const double* Minv; const double* b; };
+
+// Host driver of k_pcg<BS>: launch shape, work vectors, coarse buffers and the cooperative launch.  The caller chooses the coarse
+// space (node count, prolongation) and when its inverse is rebuilt (coarse_mode of each launch).
+template <int BS>
+struct PcgDriver {
+  int n = 0, block = 0, grid = 0;     // block rows, CTA size, CTAs
+  void* fn = nullptr;                 // the k_pcg instantiation for `block`
+  int agg = 0, nc = 0, prolong = 0;   // coarse level (PcgArgs); agg == 0: none
+  PcgSystem sys{};                    // what every launch solves (alloc)
+  DevBuf<double> x, r, z, p, q, partials, status, Ac, rc, yc;
+  DevBuf<unsigned> bar;
+
+  int nC() const { return agg > 0 ? BS * nc : 0; }
+
+  // One warp per block row: one 512-thread CTA per SM (one grid-barrier participant per SM) when the rows fill the chip, else
+  // 256-thread CTAs, two per SM, to spread a small system over many SMs.  At most nc_max coarse nodes (0: none).  No allocation.
+  void shape(int rows, int nc_max, int prolong_) {
+    n = rows;
+    block = ((long long)n * 32 >= (long long)sm_count() * PCG_TPB) ? 512 : 256;
+    fn = block == 512 ? (void*)k_pcg<BS, 512, 1> : (void*)k_pcg<BS, 256, 2>;
+    int per_sm = 0;
+    CCM_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, (const void*)fn, block, 0));
+    CCM_REQUIRE(per_sm >= 1, "k_pcg does not fit on an SM");
+    per_sm = std::min(per_sm, block == 256 ? 2 : 1);
+    grid = std::max(1, std::min(sm_count() * per_sm, div_up((long long)std::max(n, 1) * 32, block)));
+    prolong = prolong_;
+    pcg_coarse_shape(n, nc_max, &agg, &nc);
+  }
+
+  // the system's buffers must stay where they are while the driver launches
+  void alloc(const PcgSystem& system, cudaStream_t s) {
+    sys = system;
+    const size_t nv = std::max((size_t)n * BS, (size_t)1), cn = (size_t)BS * nc;
+    x.alloc_zero(nv, s); r.alloc(nv); z.alloc(nv); p.alloc(2 * nv); q.alloc(nv);
+    status.alloc_zero(4, s); bar.alloc_zero(2, s); partials.alloc((size_t)3 * grid);
+    Ac.alloc(std::max(2 * cn * cn, (size_t)1)); rc.alloc(std::max(2 * cn, (size_t)1)); yc.alloc(std::max(cn, (size_t)1));
+  }
+
+  // max_iter = 0: the coarse set-up alone; prof: PcgArgs::prof
+  void launch(double tol, int max_iter, int coarse_mode, long long* prof, cudaStream_t s) {
+    PcgArgs a;
+    a.n = n; a.rowptr = sys.rowptr; a.col = sys.col; a.val = sys.val; a.Minv = sys.Minv; a.b = sys.b;
+    a.x = x.p; a.r = r.p; a.z = z.p; a.p = p.p; a.q = q.p; a.partials = partials.p; a.bar = bar.p;
+    a.tol = tol; a.max_iter = max_iter; a.status = status.p;
+    a.agg = agg; a.nc = nc; a.coarse_mode = coarse_mode; a.prolong = prolong; a.Ac = Ac.p; a.rc = rc.p; a.yc = yc.p; a.prof = prof;
+    CCM_CUDA(cudaMemsetAsync(bar.p, 0, 2 * sizeof(unsigned), s));
+    void* args[] = {&a};
+    CCM_CUDA(cudaLaunchCooperativeKernel(fn, dim3(grid), dim3(block), args, 0, s));
+    CCM_LAUNCHED();
+  }
+};
 
 }  // namespace ccm

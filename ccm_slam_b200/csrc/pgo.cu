@@ -11,10 +11,10 @@
 #include <algorithm>
 #include <chrono>
 #include <cmath>
-#include <limits>
 
 #include "ba_math.cuh"
 #include "common.cuh"
+#include "lm_schedule.h"
 #include "pcg.cuh"
 #include "sim3_math.cuh"
 
@@ -192,15 +192,16 @@ constexpr int PGO_BIG_NC = 256;
 
 // Host-side set-up shared by ccm_pgo_solve and ccm_pgo_debug_system: the active edges (at least one free end; an edge between two
 // fixed vertices is dropped), the free-vertex index map vidx, the full symmetric block-CSR pattern of H (columns ascending), the
-// scatter slots of every active edge, the PCG CTA and grid, and the coarse shape.  n == 0 (equivalently Ea == 0): nothing to solve.
+// scatter slots of every active edge, and the PCG's shape (its buffers come with PgoDevice).  n == 0 (equivalently Ea == 0):
+// nothing to solve.
 struct PgoSetup {
   int K = 0, n = 0, Ea = 0;
   std::vector<int> vidx, rowptr, col, diag;
   std::vector<PgoEdge> edges;
   std::vector<double> meas;
   long long nnzb = 0;
-  int gsm = 0, pcg_block = 0, pcg_grid = 0, c_agg = 0, c_nc = 0, c_prolong = 0;
-  void* pcg_fn = nullptr;
+  int gsm = 0;
+  PcgDriver<7> pcg;
 
   explicit PgoSetup(const ccm_pgo_problem* p) : K(p->K) {
     const int E = p->E;
@@ -251,31 +252,22 @@ struct PgoSetup {
     }
     nnzb = (long long)col.size();
     gsm = sm_count();
-    pcg_block = ((long long)n * 32 >= (long long)gsm * PCG_TPB) ? 512 : 256;
-    pcg_fn = pcg_block == 512 ? (void*)k_pcg<7, 512, 1> : (void*)k_pcg<7, 256, 2>;
-    int per_sm = 0;
-    CCM_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, (const void*)pcg_fn, pcg_block, 0));
-    CCM_REQUIRE(per_sm >= 1, "k_pcg does not fit on an SM");
-    per_sm = std::min(per_sm, pcg_block == 256 ? 2 : 1);
-    pcg_grid = std::max(1, std::min(gsm * per_sm, div_up((long long)n * 32, pcg_block)));
     const char* env_nc = getenv("CCM_PCG_NC");
     const char* env_pl = getenv("CCM_PCG_PROLONG");
     const bool big = n >= PGO_BIG;
-    c_prolong = env_pl ? (atoi(env_pl) ? 1 : 0) : (big ? 1 : 0);
-    pcg_coarse_shape(n, env_nc ? atoi(env_nc) : (big ? PGO_BIG_NC : 64), &c_agg, &c_nc);
+    pcg.shape(n, env_nc ? atoi(env_nc) : (big ? PGO_BIG_NC : 64), env_pl ? (atoi(env_pl) ? 1 : 0) : (big ? 1 : 0));
   }
 };
 
 // Device buffers of one solve and the launches ccm_pgo_solve and ccm_pgo_debug_system share.
 struct PgoDevice {
-  const PgoSetup& S;
+  PgoSetup& S;
   cudaStream_t s;
-  DevBuf<double> d_v, d_vt, d_meas, H, Hs, b, Minv, x, pr, pz, pp, pq, partials, scal, pcg_partials, pcg_status, cAc, crc, cyc;
+  DevBuf<double> d_v, d_vt, d_meas, H, Hs, b, Minv, partials, scal;
   DevBuf<int> d_vidx, d_rowptr, d_col, d_diag, fail;
   DevBuf<PgoEdge> d_edges;
-  DevBuf<unsigned> bar;
 
-  PgoDevice(const PgoSetup& setup, const double* sim3, cudaStream_t stream) : S(setup), s(stream) {
+  PgoDevice(PgoSetup& setup, const double* sim3, cudaStream_t stream) : S(setup), s(stream) {
     const int K = S.K, n = S.n;
     const long long nnzb = S.nnzb;
     d_v.upload(sim3, (size_t)K * 8, s); d_vt.alloc((size_t)K * 8);
@@ -283,11 +275,8 @@ struct PgoDevice {
     d_vidx.upload(S.vidx.data(), K, s); d_rowptr.upload(S.rowptr.data(), n + 1, s); d_col.upload(S.col.data(), nnzb, s);
     d_diag.upload(S.diag.data(), n, s);
     H.alloc(nnzb * 49); Hs.alloc(nnzb * 49); b.alloc((size_t)n * 7); Minv.alloc((size_t)n * 49);
-    x.alloc_zero((size_t)n * 7, s); pr.alloc((size_t)n * 7); pz.alloc((size_t)n * 7); pp.alloc((size_t)2 * n * 7); pq.alloc((size_t)n * 7);
-    partials.alloc((size_t)S.gsm * 8 + 8); scal.alloc_zero(8, s); pcg_status.alloc_zero(4, s); bar.alloc_zero(2, s); fail.alloc_zero(1, s);
-    pcg_partials.alloc((size_t)3 * S.pcg_grid);
-    const size_t nC = (size_t)7 * S.c_nc;
-    cAc.alloc(std::max(2 * nC * nC, (size_t)1)); crc.alloc(std::max(2 * nC, (size_t)1)); cyc.alloc(std::max(nC, (size_t)1));
+    partials.alloc((size_t)S.gsm * 8 + 8); scal.alloc_zero(8, s); fail.alloc_zero(1, s);
+    S.pcg.alloc({d_rowptr.p, d_col.p, Hs.p, Minv.p, b.p}, s);
   }
 
   // chi2 of `state` (sum of e'e over the active edges) into dev_out
@@ -308,7 +297,7 @@ struct PgoDevice {
   }
 
   // x = (H + lambda I)^-1 b by PCG: Hs = H + lambda I, Minv = block-Jacobi inverse (fail set when a block is singular),
-  // pcg_status = [iterations, relres, flag, coarse size]
+  // S.pcg.status = [iterations, relres, flag, coarse size]
   void damped_pcg(double lambda, double tol, int max_iter) {
     const int n = S.n;
     const long long nnzb = S.nnzb;
@@ -318,15 +307,7 @@ struct PgoDevice {
     CCM_LAUNCHED();
     k_pgo_add_lambda<<<div_up(n * 7, 128), 128, 0, s>>>(Hs.p, d_diag.p, n, lambda);
     CCM_LAUNCHED();
-    CCM_CUDA(cudaMemsetAsync(bar.p, 0, 2 * sizeof(unsigned), s));
-    PcgArgs a;
-    a.n = n; a.rowptr = d_rowptr.p; a.col = d_col.p; a.val = Hs.p; a.Minv = Minv.p; a.b = b.p;
-    a.x = x.p; a.r = pr.p; a.z = pz.p; a.p = pp.p; a.q = pq.p; a.partials = pcg_partials.p; a.bar = bar.p;
-    a.tol = tol; a.max_iter = max_iter; a.status = pcg_status.p;
-    a.agg = S.c_agg; a.nc = S.c_nc; a.Ac = cAc.p; a.rc = crc.p; a.yc = cyc.p; a.coarse_mode = 1; a.prof = nullptr; a.prolong = S.c_prolong;
-    void* args[] = {&a};
-    CCM_CUDA(cudaLaunchCooperativeKernel(S.pcg_fn, dim3(S.pcg_grid), dim3(S.pcg_block), args, 0, s));
-    CCM_LAUNCHED();
+    S.pcg.launch(tol, max_iter, 1, nullptr, s);   // the coarse inverse is rebuilt on every solve
   }
 };
 
@@ -340,7 +321,7 @@ void pgo_solve(const ccm_pgo_problem* p, const ccm_pgo_options* o, ccm_pgo_resul
   const CallStream sg;
   const cudaStream_t s = sg.s;
   const int K = p->K;
-  const PgoSetup S(p);
+  PgoSetup S(p);
   const int n = S.n;
   r->trace_len = 0; r->iters_done = 0; r->chi2_initial = r->chi2_final = 0; r->lambda_final = 0;
   memcpy(r->sim3, p->sim3, sizeof(double) * 8 * K);
@@ -353,10 +334,9 @@ void pgo_solve(const ccm_pgo_problem* p, const ccm_pgo_options* o, ccm_pgo_resul
   const int pcg_max = pcg_max_of(o);
   const double pcg_tol = pcg_tol_of(o);
   auto terminate = [&] { return o->stop && *o->stop; };
-  double lambda = -1, ni = 2;
-  int nBad = 0, ret = 0;
-  bool ok = true;
-  for (int it = 0; it < o->iterations && !terminate() && ok; it++) {
+  LmSchedule lm{10};   // at most 10 trials per iteration
+  int ret = 0;
+  for (int it = 0; it < o->iterations && !terminate(); it++) {
     D.chi2_of(cur, D.scal.p);
     D.linearize(cur, p->fix_scale);
     if (it == 0 && !(o->lambda_init > 0)) {
@@ -366,61 +346,29 @@ void pgo_solve(const ccm_pgo_problem* p, const ccm_pgo_options* o, ccm_pgo_resul
     }
     CCM_CUDA(cudaMemcpyAsync(h_scal, D.scal.p, 5 * sizeof(double), cudaMemcpyDeviceToHost, s));
     CCM_CUDA(cudaStreamSynchronize(s));
-    double currentChi = h_scal[0];
-    const double iniChi = currentChi;
+    lm.begin_iteration(h_scal[0]);
     if (it == 0) {
-      r->chi2_initial = currentChi;
-      lambda = o->lambda_init > 0 ? o->lambda_init : 1e-5 * h_scal[4];
-      ni = 2; nBad = 0;
+      r->chi2_initial = h_scal[0];
+      lm.start(o->lambda_init, h_scal[4]);
     }
-    double rho = 0, tempChi = currentChi, lambda_used = lambda, relres = 0;
-    int qmax = 0, pcg_it = 0;
     do {
-      lambda_used = lambda;
-      D.damped_pcg(lambda, pcg_tol, pcg_max);
+      D.damped_pcg(lm.lambda, pcg_tol, pcg_max);
       const int g = std::max(1, std::min(div_up(K, 128), S.gsm * 8));
-      k_pgo_update<<<g, 128, 0, s>>>(cur, D.d_vidx.p, D.x.p, D.b.p, K, p->fix_scale, lambda, trial, D.partials.p);
+      k_pgo_update<<<g, 128, 0, s>>>(cur, D.d_vidx.p, S.pcg.x.p, D.b.p, K, p->fix_scale, lm.lambda, trial, D.partials.p);
       CCM_LAUNCHED();
       k_sum<<<1, 1024, 0, s>>>(D.partials.p, g, D.scal.p + 1);
       CCM_LAUNCHED();
       D.chi2_of(trial, D.scal.p + 2);
       CCM_CUDA(cudaMemcpyAsync(h_scal, D.scal.p, 3 * sizeof(double), cudaMemcpyDeviceToHost, s));
-      CCM_CUDA(cudaMemcpyAsync(h_scal + 3, D.pcg_status.p, 3 * sizeof(double), cudaMemcpyDeviceToHost, s));
+      CCM_CUDA(cudaMemcpyAsync(h_scal + 3, S.pcg.status.p, 3 * sizeof(double), cudaMemcpyDeviceToHost, s));
       CCM_CUDA(cudaMemcpyAsync(h_scal + 6, D.fail.p, sizeof(int), cudaMemcpyDeviceToHost, s));
       CCM_CUDA(cudaStreamSynchronize(s));
       int jfail;
       memcpy(&jfail, h_scal + 6, sizeof(int));
-      tempChi = h_scal[2];
-      pcg_it = (int)h_scal[3]; relres = h_scal[4];
-      const bool ok2 = !((int)h_scal[5] == 2 || jfail);
-      if (!ok2) tempChi = std::numeric_limits<double>::max();
-      rho = currentChi - tempChi;
-      double scale = h_scal[1];
-      scale += 1e-3;
-      rho /= scale;
-      if (rho > 0 && std::isfinite(tempChi)) {
-        double alpha = 1. - std::pow((2 * rho - 1), 3);
-        alpha = std::min(alpha, 2. / 3.);
-        lambda *= std::max(1. / 3., alpha);
-        ni = 2;
-        currentChi = tempChi;
-        std::swap(cur, trial);
-      } else {
-        lambda *= ni;
-        ni *= 2;
-      }
-      qmax++;
-    } while (rho < 0 && qmax < 10 && !terminate());
+      if (lm.trial(h_scal[2], h_scal[1], !((int)h_scal[5] == 2 || jfail), (int)h_scal[3], h_scal[4])) std::swap(cur, trial);
+    } while (lm.retry() && !terminate());
     ret++;
-    if (r->trace && r->trace_len < r->trace_cap) {
-      double* tr = r->trace + (size_t)r->trace_len * CCM_TRACE_COLS;
-      tr[0] = it; tr[1] = lambda_used; tr[2] = currentChi; tr[3] = rho; tr[4] = qmax; tr[5] = lambda; tr[6] = pcg_it; tr[7] = relres;
-      r->trace_len++;
-    }
-    r->chi2_final = currentChi; r->lambda_final = lambda;
-    if (qmax == 10 || rho == 0) { ok = false; continue; }
-    if ((iniChi - currentChi) * 1e3 < iniChi) nBad++; else nBad = 0;
-    if (nBad >= 3) { ok = false; continue; }
+    if (lm.end_iteration(r, it)) break;
   }
   r->iters_done = ret;
   CCM_CUDA(cudaMemcpyAsync(r->sim3, cur, sizeof(double) * 8 * K, cudaMemcpyDeviceToHost, s));
@@ -495,12 +443,12 @@ void pgo_debug_system(const ccm_pgo_problem* p, const ccm_pgo_options* o, double
                       double* pcg, int32_t* paths) {
   ensure_device();
   CCM_REQUIRE(p && o && n_free && nnzb && p->K > 0 && p->E >= 0 && p->sim3 && p->fixed, "ccm_pgo_debug_system: bad argument");
-  const PgoSetup S(p);
+  PgoSetup S(p);
   *n_free = S.n; *nnzb = S.nnzb;
   if (vidx) memcpy(vidx, S.vidx.data(), sizeof(int32_t) * S.K);
   if (rowptr) memcpy(rowptr, S.rowptr.data(), sizeof(int32_t) * (S.n + 1));
   if (col && S.nnzb) memcpy(col, S.col.data(), sizeof(int32_t) * S.nnzb);
-  if (paths) { paths[0] = S.pcg_block; paths[1] = S.c_agg; paths[2] = S.c_nc; paths[3] = 0; }
+  if (paths) { paths[0] = S.pcg.block; paths[1] = S.pcg.agg; paths[2] = S.pcg.nc; paths[3] = 0; }
   if (!H || S.n == 0) return;
   CCM_REQUIRE(b && Minv && x && chi2 && pcg, "ccm_pgo_debug_system: bad argument");
   const CallStream sg;
@@ -509,7 +457,7 @@ void pgo_debug_system(const ccm_pgo_problem* p, const ccm_pgo_options* o, double
   D.linearize(D.d_v.p, p->fix_scale);
   D.damped_pcg(lambda, pcg_tol_of(o), pcg_max_of(o));
   D.H.download(H, (size_t)S.nnzb * 49, sg.s); D.b.download(b, (size_t)S.n * 7, sg.s); D.Minv.download(Minv, (size_t)S.n * 49, sg.s);
-  D.x.download(x, (size_t)S.n * 7, sg.s); D.scal.download(chi2, 1, sg.s); D.pcg_status.download(pcg, 4, sg.s);
+  S.pcg.x.download(x, (size_t)S.n * 7, sg.s); D.scal.download(chi2, 1, sg.s); S.pcg.status.download(pcg, 4, sg.s);
   CCM_CUDA(cudaStreamSynchronize(sg.s));
   if (paths) paths[3] = pcg[3] > 0;
 }

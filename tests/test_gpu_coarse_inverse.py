@@ -79,7 +79,6 @@ CASES = [
     ("nC1536", "cfg5_768", {"CCM_PCG_IMPL": "2", "CCM_PCG_NC": "256"}, 256),
     ("nC2304", "cfg5_768", {"CCM_PCG_IMPL": "2", "CCM_PCG_NC": "384"}, 384),
     ("setup512", "cfg5_4500", {}, coarse_shape(4499, 256)[1]),
-    ("setup1024", "cfg5_4500", {"CCM_PCG_IMPL": "1", "CCM_PCG_BLOCK": "1024"}, coarse_shape(4499, 256)[1]),
 ]
 
 

@@ -1,7 +1,7 @@
 """The PCG solves of the reduced camera system, checked on the exported S and b_schur (ccm_ba_debug_schur_blocks) instead of the
 residual the kernel reports about itself: every k_pcg CTA shape, the coarse space off and on (constant and piecewise-linear
 prolongation, odd and even Gauss-Jordan sweep counts, a coarse size that is not a multiple of 8), and k_pcg2 with an odd sweep
-count and with the largest coarse system its shared memory holds (6 nc = 2304).  At K = 4500 (the 512 / 1024-thread CTAs, 256
+count and with the largest coarse system its shared memory holds (6 nc = 2304).  At K = 4500 (the 512-thread CTA, 256
 coarse nodes, refresh 4) one LM run at the default settings is also compared with the oracle."""
 import os
 import subprocess
@@ -16,7 +16,7 @@ from ccm_slam_b200 import api, synth
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GJB = 8   # pivots per Gauss-Jordan sweep (pcg.cuh)
+GJB = 32   # pivots per Gauss-Jordan sweep (pcg.cuh)
 
 
 @pytest.fixture(scope="module", autouse=True)
@@ -87,7 +87,6 @@ CASES = [
     ("k_pcg2-even-sweeps", "cfg5_tenth", {"CCM_PCG_IMPL": "2"}, 2, 256, coarse_shape(999, 128)[1]),
     ("k_pcg2-nC2304", "cfg5_768", {"CCM_PCG_IMPL": "2", "CCM_PCG_NC": "384"}, 2, 256, 384),
     ("k_pcg-512x1", "cfg5_4500", {"CCM_PCG_IMPL": "1"}, 1, 512, coarse_shape(4499, 256)[1]),
-    ("k_pcg-1024x1", "cfg5_4500", {"CCM_PCG_IMPL": "1", "CCM_PCG_BLOCK": "1024"}, 1, 1024, coarse_shape(4499, 256)[1]),
     ("k_pcg2-512-setup", "cfg5_4500", {}, 2, 512, coarse_shape(4499, 256)[1]),
 ]
 

@@ -10,7 +10,7 @@ from tests import pgo_scenes as ps
 from tests import sim3_ref as S
 
 pytestmark = pytest.mark.gpu
-GJB = 8            # pivots per Gauss-Jordan sweep of the coarse inverse (pcg.cuh)
+GJB = 32           # pivots per Gauss-Jordan sweep of the coarse inverse (pcg.cuh)
 PCG_TOL = 1e-10    # ccm_pgo_solve's defaults
 PCG_MAX = 5000
 BIG, BIG_NC = 4096, 256   # from 4096 free vertices on: 256 coarse nodes, piecewise-linear prolongation (pgo.cu)
@@ -193,8 +193,10 @@ def test_pcg_cases_cover_the_paths():
     """the cases above reach both CTA shapes, the coarse level off, nc = 1, both parities of the Gauss-Jordan sweep count and an
     aggregate size that does not divide n"""
     n = int((S.structure(ps.two_agent_merge())[1] >= 0).sum())
+    n_ragged = int((S.structure(ps.ragged())[1] >= 0).sum())
     sweeps = lambda nc: -(-7 * nc // GJB)
-    assert sweeps(coarse_shape(n, 64)[1]) % 2 == 0 and sweeps(coarse_shape(n, 3)[1]) % 2 == 1
+    # 256x2-nc64 and 256x2-ragged: the inverse ends in the second and in the first of the ping-pong buffers (coarse_inverse)
+    assert sweeps(coarse_shape(n, 64)[1]) % 2 == 1 and sweeps(coarse_shape(n_ragged, 64)[1]) % 2 == 0
     assert n % coarse_shape(n, 3)[0] != 0
     assert len(ps.tiny(2).sim3) == 2 and coarse_shape(1, 64) == (1, 1)
     assert {c[3] for c in PCG_CASES} == {256, 512}
