@@ -299,6 +299,16 @@ class BAHandle:
         _chk(lib().ccm_ba_debug_schedule(self._h, None, _p(tp), _p(sched)))
         return dict(ntasks=nt, grid=int(counts[1]), task_ptr=tp, sched=sched[:nub])
 
+    def debug_pcg2(self):
+        """k_pcg2's streamed items (ccm_ba_debug_pcg2): items (nitems, 20), cta_row / cta_item (grid+1,), slab_lo (grid, 16), streamed"""
+        counts = np.zeros(3, np.int64)
+        _chk(lib().ccm_ba_debug_pcg2(self._h, _p(counts), None, None, None, None))
+        n, g = int(counts[0]), int(counts[1])
+        items = np.empty((max(n, 1), 20), np.int32); cr = np.empty(g + 1, np.int32); ci = np.empty(g + 1, np.int32)
+        slo = np.empty((g, 16), np.int32)
+        _chk(lib().ccm_ba_debug_pcg2(self._h, None, _p(items), _p(cr), _p(ci), _p(slo)))
+        return dict(items=items[:n], cta_row=cr, cta_item=ci, slab_lo=slo, streamed=int(counts[2]))
+
     PATH_KEYS = ("pcg_impl", "pcg_block", "pcg_agg", "pcg_nc")
 
     def debug_paths(self):

@@ -94,11 +94,11 @@ struct ccm_ba_handle {
     bool window_pooled = false;
     std::vector<char*> peer;         // every rank's window as mapped here; peer[rank] == window
     DevBuf<char*> d_win;
-    DevBuf<int> items, cta_row, cta_item, rank_row;
+    DevBuf<int> items, cta_row, cta_item, rank_row, slab_lo;
     DevBuf<unsigned char> need;
     DevBuf<double> yc, tpart;
     int r0 = 0, r1 = 0, rank = 0, grid = 1;
-    long long nitems = 0;
+    long long nitems = 0, streamed = 0;
     unsigned long long launches = 0;
     long long timeout_cycles = 0;
   } p2;
@@ -284,7 +284,7 @@ void step_pcg(ccm_ba_handle* h, double tol, int max_iter) {
     if (coarse_mode == 1 && pcg.agg > 0) pcg.launch(tol, 0, coarse_mode, h->pcg_prof.p, s);
     const int nC = pcg.nC();
     Pcg2Args b;
-    b.n = h->Kf; b.val = h->s_val.p; b.items = d.items.p; b.cta_row = d.cta_row.p; b.cta_item = d.cta_item.p;
+    b.n = h->Kf; b.val = h->s_val.p; b.items = d.items.p; b.cta_row = d.cta_row.p; b.cta_item = d.cta_item.p; b.slab_lo = d.slab_lo.p;
     b.Minv = h->Minv.p; b.b = h->bschur.p; b.x = pcg.x.p; b.r = pcg.r.p; b.q = pcg.q.p; b.p = pcg.p.p;
     b.partials = pcg.partials.p; b.bar = pcg.bar.p; b.tol = tol; b.max_iter = max_iter; b.status = pcg.status.p;
     b.agg = pcg.agg; b.nc = pcg.nc; b.prolong = pcg.prolong;
@@ -339,7 +339,7 @@ void setup_pcg2(ccm_ba_handle* h, const std::vector<int>& rowptr) {
   d.r1 = rank_row[h->rank + 1];
   upload_vec(d.rank_row, rank_row, s);
   const int rows = d.r1 - d.r0;
-  // items: <= 16 consecutive blocks of one row
+  // the CTAs' rows are cut by the items of the full rows (<= 16 consecutive blocks each); pcg2_plan then builds the items streamed
   std::vector<int> row_item((size_t)rows + 1, 0);
   for (int a = 0; a < rows; a++) row_item[a + 1] = row_item[a] + (rowptr[d.r0 + a + 1] - rowptr[d.r0 + a] + P2_ITEM_BLOCKS - 1) / P2_ITEM_BLOCKS;
   d.nitems = row_item[rows];
@@ -351,7 +351,7 @@ void setup_pcg2(ccm_ba_handle* h, const std::vector<int>& rowptr) {
   d.grid = (int)std::max<long long>(1, std::min<long long>(sm_count(), (d.nitems + P2_W - 1) / P2_W));
   d.grid = std::max(1, env_int("CCM_PCG2_GRID", d.grid));
   d.grid = std::min(d.grid, sm_count() * per_sm);
-  std::vector<int> cta_row((size_t)d.grid + 1), cta_item((size_t)d.grid + 1);
+  std::vector<int> cta_row((size_t)d.grid + 1);
   for (int c = 0; c <= d.grid; c++) {
     int a = rows;
     if (c < d.grid) {
@@ -360,19 +360,22 @@ void setup_pcg2(ccm_ba_handle* h, const std::vector<int>& rowptr) {
       a = std::min(a, rows);
     }
     cta_row[c] = d.r0 + a;
-    cta_item[c] = row_item[a];
   }
-  cta_row[0] = d.r0; cta_item[0] = 0;
-  DevBuf<int> d_row_item;
-  upload_vec(d_row_item, row_item, s);
+  cta_row[0] = d.r0;
+  std::vector<int> col((size_t)rowptr[Kf]);
+  if (!col.empty()) h->s_col.download(col.data(), col.size(), s);
+  CCM_CUDA(cudaStreamSynchronize(s));
+  const Pcg2Plan plan = pcg2_plan(rowptr, col, cta_row);
+  d.nitems = (long long)plan.items.size() / P2_REC;
+  d.streamed = plan.streamed;
+  std::vector<unsigned char> need((size_t)std::max(Kf, 1), 0);
+  for (long long m = 0; m < d.nitems; m++)
+    for (int k = 0; k < plan.items[(size_t)m * P2_REC + 1]; k++) need[plan.items[(size_t)m * P2_REC + 4 + k]] = 1;
   upload_vec(d.cta_row, cta_row, s);
-  upload_vec(d.cta_item, cta_item, s);
-  d.items.alloc(std::max<size_t>((size_t)d.nitems * P2_REC, 1));
-  d.need.alloc_zero(std::max(Kf, 1), s);
-  if (rows > 0) {
-    k_pcg2_items<<<div_up(rows, 128), 128, 0, s>>>(h->s_rowptr.p, h->s_col.p, d_row_item.p, d.r0, d.r1, d.items.p, d.need.p);
-    CCM_LAUNCHED();
-  }
+  upload_vec(d.cta_item, plan.cta_item, s);
+  upload_vec(d.slab_lo, plan.slab_lo, s);
+  upload_vec(d.items, plan.items, s);
+  upload_vec(d.need, need, s);
   d.yc.alloc_zero(std::max<size_t>((size_t)2 * nC, 1), s);
   d.tpart.alloc_zero(std::max<size_t>((size_t)2 * nC, 1), s);
   if ((size_t)3 * d.grid > h->pcg.partials.n) h->pcg.partials.alloc((size_t)3 * d.grid);
@@ -1355,6 +1358,22 @@ extern "C" int ccm_ba_debug_schedule(ccm_ba_handle* h, int32_t* counts, int32_t*
     if (counts) { counts[0] = h->ntasks; counts[1] = h->schur_grid; }
     if (task_ptr) h->task_ptr.download(task_ptr, (size_t)h->ntasks + 1, s);
     if (sched && h->nub) h->u_sched.download(sched, (size_t)h->nub, s);
+    CCM_CUDA(cudaStreamSynchronize(s));
+  });
+}
+
+extern "C" int ccm_ba_debug_pcg2(ccm_ba_handle* h, int64_t* counts, int32_t* items, int32_t* cta_row, int32_t* cta_item, int32_t* slab_lo) {
+  return guarded([&] {
+    CCM_REQUIRE(h, "null handle");
+    CCM_REQUIRE(h->p2.on, "the handle does not run k_pcg2");
+    CCM_CUDA(cudaSetDevice(h->device));
+    cudaStream_t s = h->stream;
+    const ccm_ba_handle::Pcg2& d = h->p2;
+    if (counts) { counts[0] = d.nitems; counts[1] = d.grid; counts[2] = d.streamed; }
+    if (items && d.nitems) d.items.download(items, (size_t)d.nitems * P2_REC, s);
+    if (cta_row) d.cta_row.download(cta_row, (size_t)d.grid + 1, s);
+    if (cta_item) d.cta_item.download(cta_item, (size_t)d.grid + 1, s);
+    if (slab_lo) d.slab_lo.download(slab_lo, (size_t)d.grid * P2_W, s);
     CCM_CUDA(cudaStreamSynchronize(s));
   });
 }

@@ -10,7 +10,9 @@
 //    and pulls them through its own two-stage shared-memory ring with cp.async.bulk (TMA 1-D copies) completing on an mbarrier;
 //    the copy of item m + 2 is issued as soon as item m has been consumed, and the ring is cyclic over the warp's items, so the
 //    first two items of the NEXT product are already in flight while the other phases of the iteration run (S is constant
-//    during a solve).  A lane pair multiplies one 6x6 block (18 doubles per lane, conflict-free 16-byte shared loads).
+//    during a solve).  A lane pair multiplies one 6x6 block (18 doubles per lane, conflict-free 16-byte shared loads).  Inside
+//    the CTA's own rows an upper block is applied twice from one copy (S_ab p_b and S_ab^T p_a) and its mirror is not streamed
+//    (pcg2_plan, below); the transposed products gather in per-warp shared-memory slabs that complete the rows after the product.
 //  * the search direction p = z + beta p_old of the CTA's row window (own rows +- halo, <= 512 rows) is formed once per
 //    product in shared memory; only columns outside the window (loop closures, merged maps) are gathered from L2.
 //  * three grid-wide synchronisations per iteration instead of four: the restricted residual follows the recurrence
@@ -35,6 +37,9 @@
 #pragma once
 #include <stdint.h>
 
+#include <algorithm>
+#include <vector>
+
 #include "pcg.cuh"
 
 namespace ccm {
@@ -46,15 +51,19 @@ constexpr int P2_ITEM_DOUBLES = P2_ITEM_BLOCKS * 36;  // 576 doubles = 4608 byte
 constexpr int P2_REC = 20;                            // ints per item record: first block, #blocks, row, flags, col[16]
 constexpr int P2_WIN_ROWS = 512;                      // rows of the direction vector cached in shared memory
 constexpr int P2_MAX_NC = 2304;                       // coarse unknowns the shared-memory copy of rc holds (384 nodes x 6)
-constexpr size_t P2_SMEM_BYTES = (size_t)(P2_W * 2 * P2_ITEM_DOUBLES + P2_MAX_NC + P2_WIN_ROWS * 6 + P2_W * 2 * 6) * sizeof(double) +
+constexpr int P2_SLAB_ROWS = 48;                      // rows of a warp's transposed-product slab (what is left of 227 KB)
+constexpr int P2_NO_SLAB = -(1 << 30);                // slab_lo of a warp without transposed blocks
+constexpr size_t P2_SMEM_BYTES = (size_t)(P2_W * 2 * P2_ITEM_DOUBLES + P2_MAX_NC + P2_WIN_ROWS * 6 + P2_W * 2 * 6 +
+                                          P2_W * P2_SLAB_ROWS * 6) * sizeof(double) +
                                  (size_t)(P2_W * 2 + P2_W) * sizeof(int) + (size_t)(P2_W * 2) * sizeof(uint64_t);
 
 struct Pcg2Args {
   int n;                       // block rows of S
   const double* val;           // block-CSR values (all rows)
-  const int* items;            // item records of the OWN rows, P2_REC ints each, row-major order
+  const int* items;            // item records of the OWN rows, P2_REC ints each, row-major order (pcg2_plan)
   const int* cta_row;          // [grid + 1] first own row of every CTA (absolute row indices), cta_row[grid] = r1
   const int* cta_item;         // [grid + 1] first item of every CTA
+  const int* slab_lo;          // [grid * P2_W] first row of every warp's transposed-product slab, P2_NO_SLAB if it has none
   const double* Minv; const double* b;
   double *x, *r, *q, *p;       // p: 2 * n * 6
   double* partials;            // 3 * grid
@@ -84,9 +93,16 @@ __device__ __forceinline__ void p2_mbar_init(uint64_t* bar, int count) {
 __device__ __forceinline__ void p2_mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(p2_smem_u32(bar)), "r"(bytes) : "memory");
 }
-__device__ __forceinline__ void p2_bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(p2_smem_u32(dst)),
-               "l"(src), "r"(bytes), "r"(p2_smem_u32(bar))
+// S is read once per product and evicted first, so that the coarse inverse and the vectors, read every iteration, stay in L2
+__device__ __forceinline__ uint64_t p2_evict_first_policy() {
+  uint64_t pol;
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+  return pol;
+}
+__device__ __forceinline__ void p2_bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar, uint64_t pol) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(
+                   p2_smem_u32(dst)),
+               "l"(src), "r"(bytes), "r"(p2_smem_u32(bar)), "l"(pol)
                : "memory");
 }
 __device__ __forceinline__ bool p2_mbar_try_wait(uint64_t* bar, uint32_t parity) {
@@ -254,6 +270,8 @@ __global__ void __launch_bounds__(P2_TPB, 1) k_pcg2(Pcg2Args A) {
   int* sm_brow = reinterpret_cast<int*>(sm_bval + P2_W * 2 * 6);  // [W][2]
   int* sm_bcnt = sm_brow + P2_W * 2;                      // [W]
   uint64_t* sm_mbar = reinterpret_cast<uint64_t*>(sm_bcnt + P2_W);  // [W][2]
+  double* sm_slab = reinterpret_cast<double*>(sm_mbar + P2_W * 2);   // [W][P2_SLAB_ROWS * 6] transposed products S_ab^T p_a at row b
+  __shared__ int s_slo[P2_W];
   __shared__ double red[P2_TPB / 32];
   __shared__ int s_ok;
 
@@ -307,6 +325,9 @@ __global__ void __launch_bounds__(P2_TPB, 1) k_pcg2(Pcg2Args A) {
   const int nwi = we - wb;
   double* ring = sm_ring + (size_t)wid * 2 * P2_ITEM_DOUBLES;
   uint64_t* mb = sm_mbar + wid * 2;
+  double* slab = sm_slab + (size_t)wid * P2_SLAB_ROWS * 6;
+  const int slo = A.slab_lo[(size_t)blockIdx.x * P2_W + wid];
+  if (lane == 0) s_slo[wid] = slo;
   // direction window: the block columns this CTA's items touch (one pass over its records), at most P2_WIN_ROWS rows around its own rows
   __shared__ int s_cmin, s_cmax;
   if (tid == 0) { s_cmin = A.n; s_cmax = -1; }
@@ -348,12 +369,13 @@ __global__ void __launch_bounds__(P2_TPB, 1) k_pcg2(Pcg2Args A) {
     if (nwi <= 0 || lane >= P2_REC) return 0;
     return __ldg(A.items + (size_t)(wb + (int)(m % (unsigned)nwi)) * P2_REC + lane);
   };
+  const uint64_t pol = p2_evict_first_policy();
   auto issue = [&](unsigned m, int rec) {  // copy of running index m into ring buffer m & 1; lane 0 issues
     const int j0 = __shfl_sync(0xffffffffu, rec, 0), nb = __shfl_sync(0xffffffffu, rec, 1);
     if (lane == 0) {
       const uint32_t bytes = (uint32_t)nb * BB * sizeof(double);
       p2_mbar_expect_tx(mb + (m & 1u), bytes);
-      p2_bulk_g2s(ring + (size_t)(m & 1u) * P2_ITEM_DOUBLES, A.val + (size_t)j0 * BB, bytes, mb + (m & 1u));
+      p2_bulk_g2s(ring + (size_t)(m & 1u) * P2_ITEM_DOUBLES, A.val + (size_t)j0 * BB, bytes, mb + (m & 1u), pol);
     }
   };
   unsigned mrun = 0;  // running index of the next item this warp consumes
@@ -408,6 +430,11 @@ __global__ void __launch_bounds__(P2_TPB, 1) k_pcg2(Pcg2Args A) {
         const size_t g = (size_t)col * BS + k;
         return fma(beta, __ldcg(pold + g), load_z(par, g));
       };
+      for (int i = lane; i < P2_SLAB_ROWS * 6; i += 32) slab[i] = 0.0;
+      __syncwarp();
+      auto row_part = [&](int a, double yv) {  // lanes 0..5: the streamed part of (S p)_a, completed after the CTA's product
+        if (lane < BS) A.q[(size_t)a * BS + lane] = yv;
+      };
       P2CoarseAcc cs{-1, 0.0, 0.0};
       auto row_done = [&](int a, double yv) {  // lanes 0..5 hold the components of (S p)_a
         if (lane < BS) {
@@ -433,6 +460,7 @@ __global__ void __launch_bounds__(P2_TPB, 1) k_pcg2(Pcg2Args A) {
       for (int k = 0; k < nwi; k++, mrun++) {
         const int nb = __shfl_sync(0xffffffffu, rec0, 1), row = __shfl_sync(0xffffffffu, rec0, 2);
         const int flags = __shfl_sync(0xffffffffu, rec0, 3);
+        const int colb = __shfl_sync(0xffffffffu, rec0, 4 + blk);
         // next item's direction components and the record three items ahead, requested before the wait
         double pn0 = 0.0, pn1 = 0.0, pn2 = 0.0;
         if (k + 1 < nwi) {
@@ -456,6 +484,26 @@ __global__ void __launch_bounds__(P2_TPB, 1) k_pcg2(Pcg2Args A) {
           y1 += b0.x * v0 + b0.y * v1 + b1.x * v2 + b1.y * v3 + b2.x * v4 + b2.y * v5;
           y2 += d0.x * v0 + d0.y * v1 + d1.x * v2 + d1.y * v3 + d2.x * v4 + d2.y * v5;
         }
+        if (flags >> 4) {  // S_ab^T p_a for row b from the same copy: this half sums its three rows, the pair swaps halves of the result
+          const bool tr = blk < nb && ((flags >> (4 + blk)) & 1);
+          double t0 = 0.0, t1 = 0.0, t2 = 0.0, t3 = 0.0, t4 = 0.0, t5 = 0.0;
+          if (tr) {
+            const double2* sb = reinterpret_cast<const double2*>(ring + (size_t)buf * P2_ITEM_DOUBLES + (size_t)blk * BB + half * 18);
+            const double2 a0 = sb[0], a1 = sb[1], a2 = sb[2], b0 = sb[3], b1 = sb[4], b2 = sb[5], d0 = sb[6], d1 = sb[7], d2 = sb[8];
+            const double r0 = pvec(row, 3 * half), r1 = pvec(row, 3 * half + 1), r2 = pvec(row, 3 * half + 2);
+            t0 = a0.x * r0 + b0.x * r1 + d0.x * r2; t1 = a0.y * r0 + b0.y * r1 + d0.y * r2;
+            t2 = a1.x * r0 + b1.x * r1 + d1.x * r2; t3 = a1.y * r0 + b1.y * r1 + d1.y * r2;
+            t4 = a2.x * r0 + b2.x * r1 + d2.x * r2; t5 = a2.y * r0 + b2.y * r1 + d2.y * r2;
+          }
+          const double s0 = __shfl_xor_sync(0xffffffffu, half ? t0 : t3, 1), s1 = __shfl_xor_sync(0xffffffffu, half ? t1 : t4, 1),
+                       s2 = __shfl_xor_sync(0xffffffffu, half ? t2 : t5, 1);
+          if (tr) {  // the blocks of an item sit in distinct columns: no two lane pairs add into the same row
+            double* d = slab + (size_t)(colb - slo) * BS + 3 * half;
+            d[0] += (half ? t3 : t0) + s0;
+            d[1] += (half ? t4 : t1) + s1;
+            d[2] += (half ? t5 : t2) + s2;
+          }
+        }
         __syncwarp();
         issue(mrun + 2, rec2);  // the buffer just consumed takes the item two ahead (cyclic: wraps into the next product)
         if ((flags & 2) || k == nwi - 1) {
@@ -469,7 +517,7 @@ __global__ void __launch_bounds__(P2_TPB, 1) k_pcg2(Pcg2Args A) {
           const double t0 = __shfl_sync(0xffffffffu, y0, src), t1 = __shfl_sync(0xffffffffu, y1, src), t2 = __shfl_sync(0xffffffffu, y2, src);
           const double yv = (lane % 3 == 0) ? t0 : (lane % 3 == 1) ? t1 : t2;
           if (started && (flags & 2)) {
-            row_done(row, yv);
+            row_part(row, yv);
           } else {  // the row continues in a neighbouring warp's run: leave the partial sum for the merge below
             if (lane < BS) sm_bval[(size_t)(wid * 2 + npart) * BS + lane] = yv;
             if (lane == 0) sm_brow[wid * 2 + npart] = row;
@@ -481,11 +529,9 @@ __global__ void __launch_bounds__(P2_TPB, 1) k_pcg2(Pcg2Args A) {
         rec0 = rec1; rec1 = rec2; rec2 = rec3;
         pa0 = pn0; pa1 = pn1; pa2 = pn2;
       }
-      if (coarse) { p2_cflush(A, tp, cs.cur, cs.l, lane); p2_cflush(A, tp, cs.cur + 1, cs.h, lane); }
       if (lane == 0) sm_bcnt[wid] = npart;
       __syncthreads();
-      {  // rows cut by run boundaries: the warp that holds the first piece of a row sums the pieces in run order and finishes the row
-        cs = P2CoarseAcc{-1, 0.0, 0.0};
+      {  // rows cut by run boundaries: the warp that holds the first piece of a row sums the pieces in run order
         const int mycnt = sm_bcnt[wid];
         for (int e = 0; e < mycnt; e++) {
           const int row = sm_brow[wid * 2 + e];
@@ -503,10 +549,24 @@ __global__ void __launch_bounds__(P2_TPB, 1) k_pcg2(Pcg2Args A) {
             if (lane < BS) accv += sm_bval[(size_t)(w * 2 + f) * BS + lane];
             f++;
           }
-          row_done(row, accv);
+          row_part(row, accv);
         }
-        if (coarse) { p2_cflush(A, tp, cs.cur, cs.l, lane); p2_cflush(A, tp, cs.cur + 1, cs.h, lane); }
       }
+      __syncthreads();
+      // every row of the CTA: its streamed part plus the warps' transposed products in warp order (a fixed order); rows in
+      // increasing order per warp, so the running sums of P^T q apply
+      for (int a = c0 + wid; a < c1; a += P2_W) {
+        double v = 0.0;
+        if (lane < BS) {
+          v = A.q[(size_t)a * BS + lane];
+          for (int w = 0; w < P2_W; w++) {
+            const int o = a - s_slo[w];
+            if (o >= 0 && o < P2_SLAB_ROWS) v += sm_slab[((size_t)w * P2_SLAB_ROWS + o) * BS + lane];
+          }
+        }
+        row_done(a, v);
+      }
+      if (coarse) { p2_cflush(A, tp, cs.cur, cs.l, lane); p2_cflush(A, tp, cs.cur + 1, cs.h, lane); }
       if (N > 1)
         for (size_t i = g_first; i < nv; i += gstride) {
           const int a = (int)(i / BS);
@@ -710,24 +770,108 @@ inline Pcg2Layout pcg2_layout(int n, int nranks, int nC) {
   return L;
 }
 
-// item records of the rows [r0, r1): one thread per row
-__global__ void k_pcg2_items(const int* __restrict__ rowptr, const int* __restrict__ col, const int* __restrict__ row_item, int r0, int r1,
-                             int* __restrict__ items, unsigned char* __restrict__ need) {
-  const int a = r0 + blockIdx.x * blockDim.x + threadIdx.x;
-  if (a >= r1) return;
-  const int beg = rowptr[a], end = rowptr[a + 1];
-  int it = row_item[a - r0];
-  for (int j = beg; j < end; j += P2_ITEM_BLOCKS, it++) {
-    int* rec = items + (size_t)it * P2_REC;
-    const int nb = end - j < P2_ITEM_BLOCKS ? end - j : P2_ITEM_BLOCKS;
-    rec[0] = j; rec[1] = nb; rec[2] = a;
-    rec[3] = (j == beg ? 1 : 0) | (j + P2_ITEM_BLOCKS >= end ? 2 : 0);
-    for (int k = 0; k < P2_ITEM_BLOCKS; k++) {
-      const int c = k < nb ? col[j + k] : 0;
-      rec[4 + k] = c;
-      if (k < nb) need[c] = 1;   // (many writers, one value)
+// The item records of the rows [cta_row[0], cta_row[grid]) as k_pcg2 streams them (tools/pcg2_bytes.py restates this in numpy).
+// A CTA owns the rows [c0, c1).  The lane pair that holds an upper block (a, b) with a < b < c1 applies it twice: S_ab p_b for row a
+// and S_ab^T p_a for row b, into its warp's slab (flag bit 4 + k of the item).  The mirror (b, a) is then not streamed, so row b
+// streams two contiguous runs of s_val: [rowptr[b], first block at column >= c0) and [first block at column >= b, rowptr[b + 1]).
+// A warp's slab covers P2_SLAB_ROWS rows from the lowest row it adds into; a block whose row b falls beyond it is not applied
+// transposed and its mirror is streamed as before.  That changes the item counts and so the warps' runs, so the CTA's plan is
+// redone until no block falls out (blocks only ever go back to the full stream: it ends).  Nothing of it crosses a CTA, so the
+// CTAs are planned one after the other, each to its own fixed point.
+struct Pcg2Plan {
+  std::vector<int> items, cta_item, slab_lo;
+  long long streamed = 0;   // blocks streamed per product
+};
+// one CTA's rows [c0, c1): its items (appended to items), its warps' slabs (slab_lo[P2_W]); returns the blocks it streams.
+// mirror / skip / cur are scratch, reused from CTA to CTA.
+inline long long pcg2_plan_cta(const std::vector<int>& rowptr, const int* cl, int c0, int c1, std::vector<int>& items, int* slab_lo,
+                               std::vector<int>& mirror, std::vector<unsigned char>& skip, std::vector<int>& cur) {
+  const int base = rowptr[c0];
+  const size_t item0 = items.size();
+  // mirror[j - base]: the index of the mirror of upper block j when j is applied transposed, else -1; skip: that mirror
+  mirror.assign((size_t)(rowptr[c1] - base), -1);
+  skip.assign(mirror.size(), 0);
+  // merge walk: as the rows a are visited in increasing order, the mirrors (b, a) with c0 <= a < b come in increasing order in
+  // row b, so a cursor per row, started at its first column >= c0, finds each in one step
+  cur.resize((size_t)(c1 - c0));
+  for (int b = c0; b < c1; b++) cur[b - c0] = (int)(std::lower_bound(cl + rowptr[b], cl + rowptr[b + 1], c0) - cl);
+  for (int a = c0; a < c1; a++)
+    for (int j = rowptr[a]; j < rowptr[a + 1]; j++) {
+      const int b = cl[j];
+      if (b <= a) continue;
+      if (b >= c1) break;
+      const int m = cur[b - c0]++;
+      mirror[j - base] = m;
+      skip[m - base] = 1;
     }
+  for (;;) {
+    items.resize(item0);
+    long long streamed = 0;
+    for (int a = c0; a < c1; a++) {
+      const size_t first = items.size();
+      for (int j = rowptr[a]; j < rowptr[a + 1];) {
+        if (skip[j - base]) { j++; continue; }
+        int e = j;
+        while (e < rowptr[a + 1] && e - j < P2_ITEM_BLOCKS && !skip[e - base]) e++;
+        const size_t o = items.size();
+        items.resize(o + P2_REC, 0);
+        int* rec = &items[o];
+        rec[0] = j; rec[1] = e - j; rec[2] = a;
+        for (int k = 0; k < e - j; k++) {
+          rec[4 + k] = cl[j + k];
+          if (mirror[j + k - base] >= 0) rec[3] |= 1 << (4 + k);
+        }
+        streamed += e - j;
+        j = e;
+      }
+      if (items.size() > first) {
+        items[first + 3] |= 1;
+        items[items.size() - P2_REC + 3] |= 2;
+      }
+    }
+    // the warps' runs as k_pcg2 cuts them, their slabs, and the blocks that fall out of them
+    const int n = (int)((items.size() - item0) / P2_REC);
+    const int* recs = items.data() + item0;
+    bool changed = false;
+    for (int w = 0; w < P2_W; w++) {
+      const int wb = (int)((long long)n * w / P2_W), we = (int)((long long)n * (w + 1) / P2_W);
+      int lo = INT32_MAX;
+      for (int m = wb; m < we; m++) {
+        const int* rec = recs + (size_t)m * P2_REC;
+        for (int k = 0; k < rec[1]; k++)
+          if ((rec[3] >> (4 + k)) & 1) lo = std::min(lo, rec[4 + k]);
+      }
+      slab_lo[w] = lo == INT32_MAX ? P2_NO_SLAB : lo;
+      if (lo == INT32_MAX) continue;
+      for (int m = wb; m < we; m++) {
+        const int* rec = recs + (size_t)m * P2_REC;
+        for (int k = 0; k < rec[1]; k++)
+          if (((rec[3] >> (4 + k)) & 1) && rec[4 + k] - lo >= P2_SLAB_ROWS) {
+            int& mj = mirror[rec[0] + k - base];
+            skip[mj - base] = 0;
+            mj = -1;
+            changed = true;
+          }
+      }
+    }
+    if (!changed) return streamed;
   }
+}
+inline Pcg2Plan pcg2_plan(const std::vector<int>& rowptr, const std::vector<int>& col, const std::vector<int>& cta_row) {
+  const int grid = (int)cta_row.size() - 1;
+  Pcg2Plan P;
+  P.items.reserve(((size_t)(rowptr[cta_row[grid]] - rowptr[cta_row[0]]) / P2_ITEM_BLOCKS + 2 * (size_t)(cta_row[grid] - cta_row[0]) + 1) *
+                  P2_REC);
+  P.cta_item.assign((size_t)grid + 1, 0);
+  P.slab_lo.assign((size_t)grid * P2_W, P2_NO_SLAB);
+  std::vector<int> mirror, cur;
+  std::vector<unsigned char> skip;
+  for (int c = 0; c < grid; c++) {
+    P.cta_item[c] = (int)(P.items.size() / P2_REC);
+    P.streamed += pcg2_plan_cta(rowptr, col.data(), cta_row[c], cta_row[c + 1], P.items, &P.slab_lo[(size_t)c * P2_W], mirror, skip, cur);
+  }
+  P.cta_item[grid] = (int)(P.items.size() / P2_REC);
+  return P;
 }
 
 }  // namespace ccm

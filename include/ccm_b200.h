@@ -193,6 +193,11 @@ int ccm_ba_debug_schedule(ccm_ba_handle* h, int32_t* counts /*2*/, int32_t* task
 /* the PCG path the handle runs: out[0] implementation (1 k_pcg, 2 k_pcg2), out[1] k_pcg CTA size, out[2] coarse aggregate size,
  * out[3] coarse nodes (0: no coarse space) */
 int ccm_ba_debug_paths(ccm_ba_handle* h, int32_t* out /*4*/);
+/* k_pcg2's streamed items (handles that run k_pcg2 only): counts[0] items, counts[1] CTAs, counts[2] blocks streamed per product;
+ * items[20 * m] = first block, #blocks, row, flags (1 first of row, 2 last of row, 1 << (4 + k): block k also applied transposed),
+ * 16 columns; cta_row / cta_item (CTAs + 1) the CTAs' first rows and items; slab_lo (16 per CTA) every warp's first slab row.  Call
+ * with the arrays NULL to learn the counts first.  Any output may be NULL. */
+int ccm_ba_debug_pcg2(ccm_ba_handle* h, int64_t* counts /*3*/, int32_t* items, int32_t* cta_row, int32_t* cta_item, int32_t* slab_lo);
 /* the coarse level of the PCG preconditioner on the S the last ccm_ba_debug_schur left: the assembled Galerkin matrix P^T S P and
  * its inverse as the PCG set-up computes it (nC = 6 * coarse nodes, row-major nC x nC each).  Fails when the handle has no
  * coarse space or the set-up meets a non-positive pivot. */
