@@ -49,9 +49,8 @@ struct ccm_ba_handle {
   int L0 = 0, L1 = 0, Pl = 0, El = 0;
   long long E0 = 0;
   size_t Ep = 0;
-  bool sorted_input = true;
-  std::vector<int> perm;            // landmark-sorted position -> input edge index (only if !sorted_input)
-  std::vector<uint8_t> h_flags;     // local shard, sorted order
+  std::vector<int> perm;            // landmark-grouped position -> input edge index; empty when the input came grouped
+  std::vector<uint8_t> h_flags;     // local shard, grouped order
   std::vector<int> h_pose_slot, h_slot_pose;
   int words = 0, nub = 0;
   long long nnzb = 0, nprod = 0;
@@ -145,6 +144,18 @@ int grid_stride(long long n) {
   if (g < 1) g = 1;
   return (int)g;
 }
+
+// Cut k of `parts` contiguous ranges of [0, n) balanced by the non-decreasing prefix ptr[0..n]: the first index where the prefix
+// reaches k * ptr[n] / parts, clamped to [0, n]
+int prefix_cut(const int* ptr, int n, int k, int parts) {
+  if (k <= 0) return 0;
+  if (k >= parts) return n;
+  const long long want = (long long)ptr[n] * k / parts;
+  return std::min((int)(std::lower_bound(ptr, ptr + n + 1, (int)want) - ptr), n);
+}
+
+// the caller's index of the observation at landmark-grouped position gi
+long long input_edge(const ccm_ba_handle* h, long long gi) { return h->perm.empty() ? gi : h->perm[gi]; }
 
 size_t ev_record(ccm_ba_handle* h) {
   if (h->ev_used == h->ev_pool.size()) {
@@ -325,15 +336,9 @@ void setup_pcg2(ccm_ba_handle* h, const std::vector<int>& rowptr) {
   cudaStream_t s = h->stream;
   const int N = h->nranks, Kf = h->Kf;
   d.rank = h->rank;
-  // contiguous block rows per rank, cut where the block-count prefix crosses k * nnzb / N
-  auto cut = [&](int k) {
-    if (k <= 0) return 0;
-    if (k >= N) return Kf;
-    const long long want = (long long)rowptr[Kf] * k / N;
-    return (int)(std::lower_bound(rowptr.begin(), rowptr.end(), (int)want) - rowptr.begin());
-  };
+  // contiguous block rows per rank, balanced by block count
   std::vector<int> rank_row((size_t)N + 1);
-  for (int k = 0; k <= N; k++) rank_row[k] = std::min(cut(k), Kf);
+  for (int k = 0; k <= N; k++) rank_row[k] = prefix_cut(rowptr.data(), Kf, k, N);
   for (int k = 1; k <= N; k++) rank_row[k] = std::max(rank_row[k], rank_row[k - 1]);
   d.r0 = rank_row[h->rank];
   d.r1 = rank_row[h->rank + 1];
@@ -352,16 +357,7 @@ void setup_pcg2(ccm_ba_handle* h, const std::vector<int>& rowptr) {
   d.grid = std::max(1, env_int("CCM_PCG2_GRID", d.grid));
   d.grid = std::min(d.grid, sm_count() * per_sm);
   std::vector<int> cta_row((size_t)d.grid + 1);
-  for (int c = 0; c <= d.grid; c++) {
-    int a = rows;
-    if (c < d.grid) {
-      const long long want = d.nitems * c / d.grid;
-      a = (int)(std::lower_bound(row_item.begin(), row_item.end(), (int)want) - row_item.begin());
-      a = std::min(a, rows);
-    }
-    cta_row[c] = d.r0 + a;
-  }
-  cta_row[0] = d.r0;
+  for (int c = 0; c <= d.grid; c++) cta_row[c] = d.r0 + prefix_cut(row_item.data(), rows, c, d.grid);
   std::vector<int> col((size_t)rowptr[Kf]);
   if (!col.empty()) h->s_col.download(col.data(), col.size(), s);
   CCM_CUDA(cudaStreamSynchronize(s));
@@ -454,230 +450,209 @@ void step_update_and_residual(ccm_ba_handle* h, double lambda, int robust, doubl
   h->pt_eval = h->pt_trial;
 }
 
-// landmark range [L0, L1) of `rank`: contiguous, cut where the observation prefix crosses rank * E / nranks
+// landmark range [L0, L1) of `rank`: contiguous, balanced by observation count
 void shard_range(const int* lm_ptr, int P, int rank, int nranks, int* L0, int* L1) {
-  const long long E = lm_ptr[P];
-  auto cut = [&](int r) {
-    if (r <= 0) return 0;
-    if (r >= nranks) return P;
-    const long long target = E * r / nranks;
-    return (int)(std::lower_bound(lm_ptr, lm_ptr + P + 1, (int)target) - lm_ptr);
-  };
-  *L0 = std::min(cut(rank), P);
-  *L1 = std::min(std::max(cut(rank + 1), *L0), P);
+  *L0 = prefix_cut(lm_ptr, P, rank, nranks);
+  *L1 = std::max(prefix_cut(lm_ptr, P, rank + 1, nranks), *L0);
 }
 
-// ---- structure ------------------------------------------------------------------------------------------------
-void build(ccm_ba_handle* h, const ccm_ba_problem* p) {
-  const double T0 = now_ms();
+void do_reset(ccm_ba_handle* h) {
+  cudaStream_t s = h->stream;
+  CCM_CUDA(cudaMemcpyAsync(h->pose_cur, h->pose0.p, h->pose0.bytes(), cudaMemcpyDeviceToDevice, s));
+  if (h->Pl) CCM_CUDA(cudaMemcpyAsync(h->pt_cur, h->pt0.p, sizeof(double) * 3 * h->Pl, cudaMemcpyDeviceToDevice, s));
+  h->pose_eval = h->pose_cur; h->pt_eval = h->pt_cur;
+  CCM_CUDA(cudaStreamSynchronize(s));
+}
+
+// k_check_obs over n observations: throws `what` if an index is out of range or, with w given, a weight is negative; returns whether
+// the observations come grouped by landmark
+bool check_obs(ccm_ba_handle* h, const int* kf, const int* mp, const float* w, int n, int P, const char* what) {
+  cudaStream_t s = h->stream;
+  DevBuf<int> chk; chk.alloc_zero(2, s);
+  k_check_obs<<<grid_stride(n), TPB, 0, s>>>(kf, mp, w, n, h->K, P, chk.p);
+  CCM_LAUNCHED();
+  int hc[2];
+  chk.download(hc, 2, s);
+  CCM_CUDA(cudaStreamSynchronize(s));
+  CCM_REQUIRE(hc[0] == 0, what);
+  return hc[1] == 0;
+}
+
+// the caller's edge flags (input order; null: none) on the local shard, in grouped order
+void map_edge_flags(ccm_ba_handle* h, const uint8_t* flags) {
+  h->h_flags.assign(h->El, 0);
+  for (int i = 0; flags && i < h->El; i++) h->h_flags[i] = flags[input_edge(h, h->E0 + i)];
+}
+
+// the weights the LM loop reads: the raw ones with h_flags applied (none given: every flag is 0)
+void apply_edge_flags(ccm_ba_handle* h, bool given) {
+  cudaStream_t s = h->stream;
+  const int El = h->El;
+  if (!El) return;
+  if (given) h->d_flags.upload(h->h_flags.data(), El, s);
+  else CCM_CUDA(cudaMemsetAsync(h->d_flags.p, 0, (size_t)El, s));   // no flags: nothing to send
+  k_apply_flags<<<div_up(El, TPB), TPB, 0, s>>>(h->o_w_raw.p, h->d_flags.p, El, h->o_w.p);
+  CCM_LAUNCHED();
+}
+
+// ---- structure: the phases of ccm_ba_create --------------------------------------------------------------------------------------
+// What the phases hand each other besides the handle, alive until the create ends: the device scratch is freed only after the
+// system's storage is allocated, so that storage never lands in its blocks (the PCG vectors' placement is measured: system_storage).
+// One rank: the measurements (pixel coordinates and weights, 12 of the 20 bytes per observation) travel on a second stream while the
+// structure of S is built from the index lists on the first; the LM stream waits for them just before their first reader.  The
+// stream and its event live as long as the process (a stream per handle goes through the driver's global lock and can stall for a
+// long time when something else holds it).  Builds on several threads share stream and event: a later record only makes an earlier
+// build wait for more.  The destructor drains the stream before any member goes away, the grouped host arrays it reads included.
+struct Setup {
+  std::vector<int> kf, mp;             // ungrouped input grouped by landmark on the host; empty when the input came grouped
+  std::vector<float> uv, w;
+  DevBuf<int> g_kf, g_lm, g_ptr;       // several ranks: every observation and the landmark offsets on the device
+  cudaStream_t meas = nullptr; cudaEvent_t meas_done = nullptr;   // one rank: the measurements' copy stream and its event
+  DevBuf<int> row_count;               // blocks of S per row
+  DevBuf<unsigned> cursor;             // per upper block: list lengths (count walk), then cursors (fill walk)
+  DevBuf<int> row_obs, row_obs_ptr;    // the local observations grouped by block row
+  ~Setup() { if (meas) cudaStreamSynchronize(meas); }
+};
+
+struct ObsLists { const int *kf, *lm, *ptr; };   // every observation on the device, grouped by landmark, and the landmark offsets
+
+void open_handle(ccm_ba_handle* h, const ccm_ba_problem* p) {
   ensure_device();
   h->device = current_device();
   CCM_CUDA(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
   CCM_CUDA(cudaMallocHost((void**)&h->h_scal, 16 * sizeof(double)));
-  cudaStream_t s = h->stream;
   CCM_REQUIRE(p && p->K > 0 && p->P >= 0 && p->E >= 0, "ccm_ba_create: bad sizes");
   CCM_REQUIRE(p->poses && p->intr && p->fixed && (p->P == 0 || p->points), "ccm_ba_create: null pose/point arrays");
   CCM_REQUIRE(p->E == 0 || (p->obs_kf && p->obs_mp && p->obs_uv && p->obs_w), "ccm_ba_create: null observation arrays");
   h->K = p->K; h->P = p->P; h->E = p->E;
   h->rank = comm().rank; h->nranks = comm().nranks;
-  const int K = p->K, P = p->P, E = p->E;
-  // CCM_SETUP_PROF=1: wall time of the set-up phases on stderr (each lap synchronises the stream: diagnostics only)
-  const bool sprof = env_int("CCM_SETUP_PROF", 0) != 0;
-  double t_lap = now_ms();
-  auto lap = [&](const char* what) {
-    if (!sprof) return;
-    cudaStreamSynchronize(s);
-    const double t = now_ms();
-    fprintf(stderr, "[ccm_ba_create r%d] %-28s %8.2f ms\n", h->rank, what, t - t_lap);
-    t_lap = t;
-  };
+}
 
-  // free poses
+void free_pose_slots(ccm_ba_handle* h, const ccm_ba_problem* p) {
+  cudaStream_t s = h->stream;
+  const int K = h->K;
   h->h_pose_slot.assign(K, -1);
   for (int k = 0; k < K; k++)
     if (!p->fixed[k]) { h->h_pose_slot[k] = (int)h->h_slot_pose.size(); h->h_slot_pose.push_back(k); }
   h->Kf = (int)h->h_slot_pose.size();
-  const int Kf = h->Kf;
   h->pose0.upload(p->poses, (size_t)K * 7, s);
   h->poseA.alloc((size_t)K * 7); h->poseB.alloc((size_t)K * 7);
   h->intr.upload(p->intr, (size_t)K * 4, s);
   h->pose_slot.upload(h->h_pose_slot.data(), K, s);
   upload_vec(h->slot_pose, h->h_slot_pose, s);
+}
 
-  // Observations must be grouped by landmark (the reference adds edges landmark by landmark).
-  // Fast path (single rank, already grouped): the caller's arrays go to the device as they are, validation and the
-  // landmark offsets are kernels - no host pass over the observations.  Otherwise: host counting sort + shard cut.
-  std::vector<int> g_lm_ptr, g_kf, g_lm;
-  DevBuf<int> g_dkf, g_dlm, g_dptr;  // multi-rank fast path: the global (kf, landmark) lists and landmark offsets on the device
+// Observations must be grouped by landmark (the reference adds edges landmark by landmark).  The index lists go to the device as
+// they are and are validated there; ungrouped input is grouped on the host by a stable counting sort and sent again, and from then
+// on every input takes one path.  On one rank the shard is every observation: the device lists are the global and the local ones.
+// On several ranks the shard is cut from the landmark offsets and sliced from the global lists on the device.
+ObsLists take_observations(ccm_ba_handle* h, const ccm_ba_problem* p, Setup& st) {
+  cudaStream_t s = h->stream;
+  const int P = h->P, E = h->E;
   const bool multi = h->nranks > 1;
-  // One rank, grouped input: the measurements (pixel coordinates and weights, 12 of the 20 bytes per observation) travel on a
-  // second stream while the structure of S is built from the index lists on the first; the LM stream waits for them just
-  // before their first reader (the pose observation stream).  The stream and its event live as long as the process (a stream
-  // per handle goes through the driver's global lock and can stall for a long time when something else holds it); the guard drains the stream before the caller's arrays can go away.  Builds on several threads share stream and
-  // event: a later record only makes an earlier build wait for more.  CCM_MEAS_OVERLAP=0 keeps everything on the handle's stream.
-  struct MeasCopy {
-    cudaStream_t cs = nullptr;
-    cudaEvent_t ev = nullptr;
-    bool used = false;
-    ~MeasCopy() { if (used) cudaStreamSynchronize(cs); }
-  } meas;
-  bool fast = E > 0;
-  if (fast) {
-    DevBuf<int>& dk = multi ? g_dkf : h->o_kf;
-    DevBuf<int>& dl = multi ? g_dlm : h->o_lm;
-    dk.upload(p->obs_kf, E, s); dl.upload(p->obs_mp, E, s);
-    if (!multi) {
-      if (env_int("CCM_MEAS_OVERLAP", 1)) {
-        copy_stream(&meas.cs, &meas.ev);
-        meas.used = true;
-      } else {
-        meas.cs = s;   // same stream: no overlap
-      }
-      h->o_uv.upload(reinterpret_cast<const float2*>(p->obs_uv), E, meas.cs); h->o_w_raw.upload(p->obs_w, E, meas.cs);
-      if (meas.used) CCM_CUDA(cudaEventRecord(meas.ev, meas.cs));
-    }
-    DevBuf<int> chk; chk.alloc_zero(2, s);
-    k_check_obs<<<grid_stride(E), TPB, 0, s>>>(dk.p, dl.p, nullptr, E, K, P, chk.p);   // indices here; the weights of the one-rank path below
-    CCM_LAUNCHED();
-    int hc[2];
-    chk.download(hc, 2, s);
-    CCM_CUDA(cudaStreamSynchronize(s));
-    CCM_REQUIRE(hc[0] == 0, "ccm_ba_create: observation index out of range");
-    if (hc[1] != 0) {   // not grouped by landmark: take the sorting path (which uploads the measurements in sorted order itself)
-      fast = false; g_dkf.release(); g_dlm.release();
-      if (meas.used) CCM_CUDA(cudaStreamSynchronize(meas.cs));
-    }
-  }
-  if (fast && !multi) {
-    h->sorted_input = true;
-    h->L0 = 0; h->L1 = P; h->Pl = P; h->E0 = 0; h->El = E;
-    h->Ep = ((size_t)E + 31) / 32 * 32;
-    h->lm_ptr.alloc((size_t)P + 1);
-    k_lm_ptr<<<div_up((long long)P + 1, TPB), TPB, 0, s>>>(h->o_lm.p, E, P, h->lm_ptr.p);
-    CCM_LAUNCHED();
-    if (p->edge_flags) h->h_flags.assign(p->edge_flags, p->edge_flags + E); else h->h_flags.assign(E, 0);
-  } else if (fast) {
-    // grouped input on several ranks: cut the shard from the landmark offsets (4 B per landmark come back to the host), slice
-    // the lists on the device, upload only this rank's measurements
-    h->sorted_input = true;
-    g_dptr.alloc((size_t)P + 1);
-    k_lm_ptr<<<div_up((long long)P + 1, TPB), TPB, 0, s>>>(g_dlm.p, E, P, g_dptr.p);
-    CCM_LAUNCHED();
-    std::vector<int> hp((size_t)P + 1);
-    g_dptr.download(hp.data(), hp.size(), s);
-    CCM_CUDA(cudaStreamSynchronize(s));
-    shard_range(hp.data(), P, h->rank, h->nranks, &h->L0, &h->L1);
-    h->Pl = h->L1 - h->L0;
-    h->E0 = hp[h->L0];
-    h->El = hp[h->L1] - hp[h->L0];
-    h->Ep = ((size_t)h->El + 31) / 32 * 32;
-    const int El_ = h->El, Pl_ = h->Pl;
-    h->o_kf.alloc(std::max(El_, 1)); h->o_lm.alloc(std::max(El_, 1)); h->lm_ptr.alloc((size_t)Pl_ + 1);
-    h->o_uv.alloc(std::max(El_, 1)); h->o_w_raw.alloc(std::max(El_, 1));
-    if (El_) {
-      CCM_CUDA(cudaMemcpyAsync(h->o_kf.p, g_dkf.p + h->E0, sizeof(int) * (size_t)El_, cudaMemcpyDeviceToDevice, s));
-      k_shift<<<div_up(El_, TPB), TPB, 0, s>>>(g_dlm.p + h->E0, El_, h->L0, h->o_lm.p);
-      CCM_LAUNCHED();
-      CCM_CUDA(cudaMemcpyAsync(h->o_uv.p, reinterpret_cast<const float2*>(p->obs_uv) + h->E0, sizeof(float2) * (size_t)El_, cudaMemcpyHostToDevice, s));
-      CCM_CUDA(cudaMemcpyAsync(h->o_w_raw.p, p->obs_w + h->E0, sizeof(float) * (size_t)El_, cudaMemcpyHostToDevice, s));
-      DevBuf<int> chk; chk.alloc_zero(2, s);
-      k_check_obs<<<grid_stride(El_), TPB, 0, s>>>(h->o_kf.p, h->o_lm.p, h->o_w_raw.p, El_, K, std::max(Pl_, 1), chk.p);
-      CCM_LAUNCHED();
-      int hc[2];
-      chk.download(hc, 2, s);
-      CCM_CUDA(cudaStreamSynchronize(s));
-      CCM_REQUIRE(hc[0] == 0, "ccm_ba_create: negative information weight");
-    }
-    k_shift<<<div_up((long long)Pl_ + 1, TPB), TPB, 0, s>>>(g_dptr.p + h->L0, (long long)Pl_ + 1, (int)h->E0, h->lm_ptr.p);
-    CCM_LAUNCHED();
-    if (p->edge_flags) h->h_flags.assign(p->edge_flags + h->E0, p->edge_flags + h->E0 + El_); else h->h_flags.assign(El_, 0);
-  } else {
-    bool sorted = true;
-    for (int e = 0; e < E; e++) {
-      CCM_REQUIRE(p->obs_kf[e] >= 0 && p->obs_kf[e] < K && p->obs_mp[e] >= 0 && p->obs_mp[e] < P,
-                  "ccm_ba_create: observation index out of range");
-      if (e && p->obs_mp[e] < p->obs_mp[e - 1]) sorted = false;
-    }
-    g_lm_ptr.assign((size_t)P + 1, 0);
-    for (int e = 0; e < E; e++) g_lm_ptr[p->obs_mp[e] + 1]++;
-    for (int l = 0; l < P; l++) g_lm_ptr[l + 1] += g_lm_ptr[l];
-    h->sorted_input = sorted;
-    g_kf.resize((size_t)E); g_lm.resize((size_t)E);
-    if (sorted) {
-      std::copy(p->obs_kf, p->obs_kf + E, g_kf.begin());
-      std::copy(p->obs_mp, p->obs_mp + E, g_lm.begin());
-    } else {
+  DevBuf<int>& dk = multi ? st.g_kf : h->o_kf;
+  DevBuf<int>& dl = multi ? st.g_lm : h->o_lm;
+  DevBuf<int>& dp = multi ? st.g_ptr : h->lm_ptr;
+  const int *kf = p->obs_kf, *mp = p->obs_mp;
+  const float *uv = p->obs_uv, *w = p->obs_w;
+  auto send = [&] {
+    dk.upload(kf, E, s); dl.upload(mp, E, s);
+    if (multi) return;   // several ranks send their shard's measurements once it is cut
+    copy_stream(&st.meas, &st.meas_done);
+    h->o_uv.upload(reinterpret_cast<const float2*>(uv), E, st.meas); h->o_w_raw.upload(w, E, st.meas);
+    CCM_CUDA(cudaEventRecord(st.meas_done, st.meas));
+  };
+  if (E > 0) {
+    send();
+    if (!check_obs(h, dk.p, dl.p, nullptr, E, P, "ccm_ba_create: observation index out of range")) {
+      std::vector<int> at((size_t)P + 1, 0);   // the indices are in range: the counting sort stays inside its arrays
+      for (int e = 0; e < E; e++) at[mp[e] + 1]++;
+      for (int l = 0; l < P; l++) at[l + 1] += at[l];
       h->perm.resize(E);
-      std::vector<int> cur(g_lm_ptr.begin(), g_lm_ptr.end() - 1);
-      for (int e = 0; e < E; e++) h->perm[cur[p->obs_mp[e]]++] = e;
-      for (int i = 0; i < E; i++) { g_kf[i] = p->obs_kf[h->perm[i]]; g_lm[i] = p->obs_mp[h->perm[i]]; }
+      for (int e = 0; e < E; e++) h->perm[at[mp[e]]++] = e;
+      st.kf.resize(E); st.mp.resize(E); st.uv.resize((size_t)2 * E); st.w.resize(E);
+      for (int i = 0; i < E; i++) {
+        const int e = h->perm[i];
+        st.kf[i] = kf[e]; st.mp[i] = mp[e]; st.uv[2 * i] = uv[2 * e]; st.uv[2 * i + 1] = uv[2 * e + 1]; st.w[i] = w[e];
+      }
+      kf = st.kf.data(); mp = st.mp.data(); uv = st.uv.data(); w = st.w.data();
+      send();
     }
-    auto src = [&](long long i) { return sorted ? i : (long long)h->perm[i]; };
-    // landmark shard of this rank: contiguous landmark range balanced by observation count
-    shard_range(g_lm_ptr.data(), P, h->rank, h->nranks, &h->L0, &h->L1);
-    h->Pl = h->L1 - h->L0;
-    h->E0 = g_lm_ptr[h->L0];
-    h->El = g_lm_ptr[h->L1] - g_lm_ptr[h->L0];
-    h->Ep = ((size_t)h->El + 31) / 32 * 32;
-    const int El_ = h->El, Pl_ = h->Pl;
-    std::vector<int> l_kf(El_), l_lm(El_), l_ptr((size_t)Pl_ + 1);
-    std::vector<float2> l_uv(El_);
-    std::vector<float> l_w(El_);
-    h->h_flags.assign(El_, 0);
-    for (int i = 0; i < El_; i++) {
-      const long long gi = h->E0 + i, si = src(gi);
-      l_kf[i] = g_kf[gi];
-      l_lm[i] = g_lm[gi] - h->L0;
-      l_uv[i] = make_float2(p->obs_uv[2 * si], p->obs_uv[2 * si + 1]);
-      l_w[i] = p->obs_w[si];
-      CCM_REQUIRE(l_w[i] >= 0.0f, "ccm_ba_create: negative information weight");
-      if (p->edge_flags) h->h_flags[i] = p->edge_flags[si];
-    }
-    for (int l = 0; l <= Pl_; l++) l_ptr[l] = g_lm_ptr[h->L0 + l] - (int)h->E0;
-    upload_vec(h->o_kf, l_kf, s); upload_vec(h->o_lm, l_lm, s); upload_vec(h->lm_ptr, l_ptr, s);
-    upload_vec(h->o_uv, l_uv, s); upload_vec(h->o_w_raw, l_w, s);
-    CCM_CUDA(cudaStreamSynchronize(s));  // the staging vectors die at the end of this scope
   }
-  lap("observations + shard");
+  dp.alloc((size_t)P + 1);
+  k_lm_ptr<<<div_up((long long)P + 1, TPB), TPB, 0, s>>>(dl.p, E, P, dp.p);
+  CCM_LAUNCHED();
+  const ObsLists all{dk.p, dl.p, dp.p};
+  if (!multi) {
+    h->L0 = 0; h->L1 = P; h->Pl = P; h->E0 = 0; h->El = E;
+    return all;
+  }
+  // several ranks: the shard's cut needs the landmark offsets on the host (4 B per landmark), then the lists are sliced on the device
+  // and only this rank's measurements are sent
+  std::vector<int> hp((size_t)P + 1);
+  dp.download(hp.data(), hp.size(), s);
+  CCM_CUDA(cudaStreamSynchronize(s));
+  shard_range(hp.data(), P, h->rank, h->nranks, &h->L0, &h->L1);
+  h->Pl = h->L1 - h->L0; h->E0 = hp[h->L0]; h->El = hp[h->L1] - hp[h->L0];
+  const int El = h->El, Pl = h->Pl;
+  h->o_kf.alloc(std::max(El, 1)); h->o_lm.alloc(std::max(El, 1)); h->lm_ptr.alloc((size_t)Pl + 1);
+  h->o_uv.alloc(std::max(El, 1)); h->o_w_raw.alloc(std::max(El, 1));
+  if (El) {
+    CCM_CUDA(cudaMemcpyAsync(h->o_kf.p, st.g_kf.p + h->E0, sizeof(int) * (size_t)El, cudaMemcpyDeviceToDevice, s));
+    k_shift<<<div_up(El, TPB), TPB, 0, s>>>(st.g_lm.p + h->E0, El, h->L0, h->o_lm.p);
+    CCM_LAUNCHED();
+    CCM_CUDA(cudaMemcpyAsync(h->o_uv.p, reinterpret_cast<const float2*>(uv) + h->E0, sizeof(float2) * (size_t)El, cudaMemcpyHostToDevice, s));
+    CCM_CUDA(cudaMemcpyAsync(h->o_w_raw.p, w + h->E0, sizeof(float) * (size_t)El, cudaMemcpyHostToDevice, s));
+    check_obs(h, h->o_kf.p, h->o_lm.p, h->o_w_raw.p, El, std::max(Pl, 1), "ccm_ba_create: negative information weight");
+  }
+  k_shift<<<div_up((long long)Pl + 1, TPB), TPB, 0, s>>>(st.g_ptr.p + h->L0, (long long)Pl + 1, (int)h->E0, h->lm_ptr.p);
+  CCM_LAUNCHED();
+  return all;
+}
+
+// the shard's points and the buffers of its flagged weights
+void shard_storage(ccm_ba_handle* h, const ccm_ba_problem* p) {
+  cudaStream_t s = h->stream;
   const int Pl = h->Pl, El = h->El;
+  h->Ep = ((size_t)El + 31) / 32 * 32;
   h->pt0.alloc(std::max((size_t)Pl * 3, (size_t)1));
   if (Pl) CCM_CUDA(cudaMemcpyAsync(h->pt0.p, p->points + 3 * (size_t)h->L0, sizeof(double) * 3 * Pl, cudaMemcpyHostToDevice, s));
   h->ptA.alloc(std::max((size_t)Pl * 3, (size_t)1)); h->ptB.alloc(std::max((size_t)Pl * 3, (size_t)1));
   h->o_w.alloc(std::max(El, 1)); h->d_flags.alloc(std::max(El, 1));
+}
 
-  // ---- covisibility bitmap over ALL observations (every rank needs the global pattern of S)
-  h->words = (Kf + 31) / 32;
-  const int words = std::max(h->words, 1);
-  h->words = words;
+// covisibility bitmap over ALL observations (every rank needs the global pattern of S), its per-word prefix and the blocks per row
+void covisibility_bitmap(ccm_ba_handle* h, const ObsLists& all, Setup& st) {
+  cudaStream_t s = h->stream;
+  const int Kf = h->Kf, E = h->E;
+  const int words = h->words = std::max((Kf + 31) / 32, 1);
   h->bitmap.alloc_zero((size_t)std::max(Kf, 1) * words, s);
   h->word_prefix.alloc((size_t)std::max(Kf, 1) * words);
-  DevBuf<int> row_count; row_count.alloc(std::max(Kf, 1));
-  {
-    DevBuf<int> d_gkf, d_glm, d_gptr;
-    const int *pk, *pl, *pp_;
-    if (h->nranks == 1) { pk = h->o_kf.p; pl = h->o_lm.p; pp_ = h->lm_ptr.p; }
-    else if (g_dptr.p) { pk = g_dkf.p; pl = g_dlm.p; pp_ = g_dptr.p; }
-    else {
-      d_gkf.upload(g_kf.data(), E, s); d_glm.upload(g_lm.data(), E, s); d_gptr.upload(g_lm_ptr.data(), (size_t)P + 1, s);
-      pk = d_gkf.p; pl = d_glm.p; pp_ = d_gptr.p;
-    }
-    if (Kf > 0) {
-      if (E > 0) {
-        k_pattern_bitmap<<<div_up(E, TPB), TPB, 0, s>>>(pk, pl, pp_, h->pose_slot.p, E, words, h->bitmap.p);
-        CCM_LAUNCHED();
-      }
-      k_set_diag_bits<<<div_up(Kf, TPB), TPB, 0, s>>>(Kf, words, h->bitmap.p);
-      CCM_LAUNCHED();
-      k_row_prefix<<<div_up(Kf, TPB), TPB, 0, s>>>(h->bitmap.p, Kf, words, h->word_prefix.p, row_count.p);
+  st.row_count.alloc(std::max(Kf, 1));
+  if (Kf > 0) {
+    if (E > 0) {
+      k_pattern_bitmap<<<div_up(E, TPB), TPB, 0, s>>>(all.kf, all.lm, all.ptr, h->pose_slot.p, E, words, h->bitmap.p);
       CCM_LAUNCHED();
     }
-    CCM_CUDA(cudaStreamSynchronize(s));  // temporaries die here
+    k_set_diag_bits<<<div_up(Kf, TPB), TPB, 0, s>>>(Kf, words, h->bitmap.p);
+    CCM_LAUNCHED();
+    k_row_prefix<<<div_up(Kf, TPB), TPB, 0, s>>>(h->bitmap.p, Kf, words, h->word_prefix.p, st.row_count.p);
+    CCM_LAUNCHED();
   }
-  lap("points, flags, bitmap, prefix");
-  std::vector<int> h_rowptr((size_t)Kf + 1, 0);
+}
+
+struct Pattern { std::vector<int> rowptr, udiag; };   // block rows of S, and each row's first upper block (its diagonal)
+
+// the block-CSR pattern of S, then the upper-block numbering, mirror map and diagonal positions: O(1) per pattern entry through the
+// bitmap prefix, on the device
+Pattern s_pattern(ccm_ba_handle* h, Setup& st) {
+  cudaStream_t s = h->stream;
+  const int Kf = h->Kf, words = h->words;
+  Pattern pat{std::vector<int>((size_t)Kf + 1, 0), std::vector<int>(std::max(Kf, 1), 0)};
+  std::vector<int> &h_rowptr = pat.rowptr, &h_udiag = pat.udiag;
   if (Kf > 0) {
     std::vector<int> cnt(Kf);
-    row_count.download(cnt.data(), Kf, s);
+    st.row_count.download(cnt.data(), Kf, s);
     CCM_CUDA(cudaStreamSynchronize(s));
     long long run = 0;
     for (int a = 0; a < Kf; a++) { h_rowptr[a] = (int)run; run += cnt[a]; CCM_REQUIRE(run < (1ll << 31), "S pattern too large"); }
@@ -692,10 +667,7 @@ void build(ccm_ba_handle* h, const ccm_ba_problem* p) {
                                                                   h->s_col.p, h->s_row.p);
     CCM_LAUNCHED();
   }
-  // upper-block numbering, mirror map, diagonal positions: O(1) per pattern entry through the bitmap prefix, on the device
-  std::vector<int> h_udiag(std::max(Kf, 1), 0);
   h->s_diag.alloc(std::max(Kf, 1)); h->u_diag.alloc(std::max(Kf, 1)); h->csr_u.alloc(std::max<long long>(nnzb, 1));
-  h->nub = 0;
   if (Kf > 0) {
     DevBuf<int> upper_count, u_rowstart, perr;
     upper_count.alloc(Kf); perr.alloc_zero(1, s);
@@ -719,36 +691,42 @@ void build(ccm_ba_handle* h, const ccm_ba_problem* p) {
   } else {
     h->u_row.alloc(1); h->u_col.alloc(1);
   }
-  const int nub = h->nub;
+  return pat;
+}
 
-  lap("pattern, upper index");
-  // ---- Schur product lists (local shard), in landmark order: the local observations grouped by block row (a stable radix sort keeps
-  // landmark order inside a row), then one warp per row counts, and after the scan fills, its blocks' lists (k_row_products)
+// Schur product lists (local shard) and their offsets, in landmark order: the local observations grouped by block row (a stable radix
+// sort keeps landmark order inside a row), then one warp per row counts, and after the scan fills, its blocks' lists (k_row_products)
+std::vector<unsigned> product_lists(ccm_ba_handle* h, Setup& st) {
+  cudaStream_t s = h->stream;
+  const int Kf = h->Kf, El = h->El, nub = h->nub;
   std::vector<unsigned> h_pp((size_t)nub + 1, 0);
-  DevBuf<unsigned> cursor; cursor.alloc_zero(std::max(nub, 1), s);
-  DevBuf<int> row_obs, row_obs_ptr;
+  st.cursor.alloc_zero(std::max(nub, 1), s);
+  auto row_products = [&](int fill, const unsigned* u_prod_ptr, uint2* prod) {
+    k_row_products<<<div_up((long long)Kf * 32, 128), 128, 0, s>>>(st.row_obs.p, st.row_obs_ptr.p, Kf, h->o_kf.p, h->o_lm.p, h->lm_ptr.p,
+                                                                   h->pose_slot.p, h->bitmap.p, h->word_prefix.p, h->s_rowptr.p,
+                                                                   h->s_diag.p, h->u_diag.p, nub, h->words, fill, st.cursor.p,
+                                                                   u_prod_ptr, prod);
+    CCM_LAUNCHED();
+  };
   if (El && nub) {
     {
       DevBuf<int> key, idx, key_s;
-      key.alloc(El); idx.alloc(El); key_s.alloc(El); row_obs.alloc(El); row_obs_ptr.alloc((size_t)Kf + 1);
+      key.alloc(El); idx.alloc(El); key_s.alloc(El); st.row_obs.alloc(El); st.row_obs_ptr.alloc((size_t)Kf + 1);
       k_row_keys<<<div_up(El, TPB), TPB, 0, s>>>(h->o_kf.p, h->pose_slot.p, El, Kf, key.p, idx.p);
       CCM_LAUNCHED();
       int bits = 1;
       while ((1ll << bits) <= Kf) bits++;
       size_t tb = 0;
-      CCM_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, key.p, key_s.p, idx.p, row_obs.p, El, 0, bits, s));
+      CCM_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, key.p, key_s.p, idx.p, st.row_obs.p, El, 0, bits, s));
       DevBuf<unsigned char> tmp; tmp.alloc(tb + 16);
-      CCM_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tb, key.p, key_s.p, idx.p, row_obs.p, El, 0, bits, s));
-      k_lm_ptr<<<div_up((long long)Kf + 1, TPB), TPB, 0, s>>>(key_s.p, El, Kf, row_obs_ptr.p);   // first observation of each row
+      CCM_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tb, key.p, key_s.p, idx.p, st.row_obs.p, El, 0, bits, s));
+      k_lm_ptr<<<div_up((long long)Kf + 1, TPB), TPB, 0, s>>>(key_s.p, El, Kf, st.row_obs_ptr.p);   // first observation of each row
       CCM_LAUNCHED();
       CCM_CUDA(cudaStreamSynchronize(s));   // the temporaries die here
     }
-    k_row_products<<<div_up((long long)Kf * 32, 128), 128, 0, s>>>(row_obs.p, row_obs_ptr.p, Kf, h->o_kf.p, h->o_lm.p, h->lm_ptr.p,
-                                                                   h->pose_slot.p, h->bitmap.p, h->word_prefix.p, h->s_rowptr.p,
-                                                                   h->s_diag.p, h->u_diag.p, nub, words, 0, cursor.p, nullptr, nullptr);
-    CCM_LAUNCHED();
+    row_products(0, nullptr, nullptr);
     std::vector<unsigned> c(nub);
-    cursor.download(c.data(), nub, s);
+    st.cursor.download(c.data(), nub, s);
     CCM_CUDA(cudaStreamSynchronize(s));
     unsigned long long run = 0;
     for (int u = 0; u < nub; u++) { h_pp[u] = (unsigned)run; run += c[u]; }
@@ -759,67 +737,64 @@ void build(ccm_ba_handle* h, const ccm_ba_problem* p) {
   upload_vec(h->u_prod_ptr, h_pp, s);
   h->prod.alloc(std::max<long long>(h->nprod, 1));
   if (h->nprod) {
-    CCM_CUDA(cudaMemsetAsync(cursor.p, 0, sizeof(unsigned) * nub, s));
-    k_row_products<<<div_up((long long)Kf * 32, 128), 128, 0, s>>>(row_obs.p, row_obs_ptr.p, Kf, h->o_kf.p, h->o_lm.p, h->lm_ptr.p,
-                                                                   h->pose_slot.p, h->bitmap.p, h->word_prefix.p, h->s_rowptr.p,
-                                                                   h->s_diag.p, h->u_diag.p, nub, words, 1, cursor.p, h->u_prod_ptr.p,
-                                                                   h->prod.p);
-    CCM_LAUNCHED();
+    CCM_CUDA(cudaMemsetAsync(st.cursor.p, 0, sizeof(unsigned) * nub, s));
+    row_products(1, h->u_prod_ptr.p, h->prod.p);
   }
-  // k_schur_mma's schedule: per row its upper blocks by decreasing list length (ties by block number), cut into tasks of at most
-  // SCHUR_TASK blocks of similar size
-  {
-    std::vector<int> sched((size_t)std::max(nub, 1)), tptr(1, 0);
-    for (int a = 0; a < Kf; a++) {
-      const int ub = h_udiag[a], n = (a + 1 < Kf ? h_udiag[a + 1] : nub) - ub;
-      int* r = sched.data() + ub;
-      std::iota(r, r + n, ub);
-      std::sort(r, r + n, [&](int x, int y) {
-        const unsigned nx = h_pp[x + 1] - h_pp[x], ny = h_pp[y + 1] - h_pp[y];
-        return nx != ny ? nx > ny : x < y;
-      });
-      const int parts = (n + SCHUR_TASK - 1) / SCHUR_TASK;
-      for (int k = 1; k <= parts; k++) tptr.push_back(ub + (int)((long long)n * k / parts));
-    }
-    h->ntasks = (int)tptr.size() - 1;
-    upload_vec(h->u_sched, sched, s);
-    upload_vec(h->task_ptr, tptr, s);
-    h->next_task.alloc(1);
-    int per_sm = 0;
-    CCM_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, (const void*)k_schur_mma, SCHUR_CTA, 0));
-    CCM_REQUIRE(per_sm >= 1, "k_schur_mma does not fit on an SM");
-    h->schur_grid = std::max(1, std::min(h->ntasks, sm_count()));
-    CCM_CUDA(cudaStreamSynchronize(s));   // the host vectors die at the end of this scope
-  }
-  lap("product lists");
-  // ---- measurements: wait for their copy (one-rank path), validate the weights there, apply the edge flags
-  if (El) {
-    if (fast && !multi) {
-      if (meas.used) CCM_CUDA(cudaStreamWaitEvent(s, meas.ev, 0));
-      DevBuf<int> chk; chk.alloc_zero(2, s);
-      k_check_obs<<<grid_stride(El), TPB, 0, s>>>(h->o_kf.p, h->o_lm.p, h->o_w_raw.p, El, K, std::max(P, 1), chk.p);
-      CCM_LAUNCHED();
-      int hc[2];
-      chk.download(hc, 2, s);
-      CCM_CUDA(cudaStreamSynchronize(s));
-      CCM_REQUIRE(hc[0] == 0, "ccm_ba_create: negative information weight");
-    }
-    if (p->edge_flags) h->d_flags.upload(h->h_flags.data(), El, s);
-    else CCM_CUDA(cudaMemsetAsync(h->d_flags.p, 0, (size_t)El, s));   // no flags: nothing to send
-    k_apply_flags<<<div_up(El, TPB), TPB, 0, s>>>(h->o_w_raw.p, h->d_flags.p, El, h->o_w.p);
-    CCM_LAUNCHED();
-  }
-  // packed per-pose observation stream for the pose pass
-  {
-    std::vector<unsigned> kp((size_t)Kf + 1, 0);
-    for (int a = 0; a < Kf; a++) kp[a + 1] = kp[a] + (h_pp[h_udiag[a] + 1] - h_pp[h_udiag[a]]);
-    upload_vec(h->kobs_ptr, kp, s);
-    h->kobs.alloc(std::max((size_t)kp[Kf], (size_t)1));
-    pack_pose_obs(h);
-  }
+  return h_pp;
+}
 
-  lap("pose observation stream");
-  // ---- landmark-aligned CTA schedule: unit heads (ba_kernels.cuh), numbered by an inclusive scan, cut where a head starts
+// k_schur_mma's schedule: per row its upper blocks by decreasing list length (ties by block number), cut into tasks of at most
+// SCHUR_TASK blocks of similar size
+void schur_schedule(ccm_ba_handle* h, const std::vector<int>& udiag, const std::vector<unsigned>& pp) {
+  cudaStream_t s = h->stream;
+  const int Kf = h->Kf, nub = h->nub;
+  std::vector<int> sched((size_t)std::max(nub, 1)), tptr(1, 0);
+  for (int a = 0; a < Kf; a++) {
+    const int ub = udiag[a], n = (a + 1 < Kf ? udiag[a + 1] : nub) - ub;
+    int* r = sched.data() + ub;
+    std::iota(r, r + n, ub);
+    std::sort(r, r + n, [&](int x, int y) {
+      const unsigned nx = pp[x + 1] - pp[x], ny = pp[y + 1] - pp[y];
+      return nx != ny ? nx > ny : x < y;
+    });
+    const int parts = (n + SCHUR_TASK - 1) / SCHUR_TASK;
+    for (int k = 1; k <= parts; k++) tptr.push_back(ub + (int)((long long)n * k / parts));
+  }
+  h->ntasks = (int)tptr.size() - 1;
+  upload_vec(h->u_sched, sched, s);
+  upload_vec(h->task_ptr, tptr, s);
+  h->next_task.alloc(1);
+  int per_sm = 0;
+  CCM_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, (const void*)k_schur_mma, SCHUR_CTA, 0));
+  CCM_REQUIRE(per_sm >= 1, "k_schur_mma does not fit on an SM");
+  h->schur_grid = std::max(1, std::min(h->ntasks, sm_count()));
+  CCM_CUDA(cudaStreamSynchronize(s));   // the host vectors die at the end of this scope
+}
+
+// measurements: wait for their copy (one rank, E > 0), validate the weights there, apply the edge flags
+void measurements(ccm_ba_handle* h, const ccm_ba_problem* p, const Setup& st) {
+  if (st.meas) {
+    CCM_CUDA(cudaStreamWaitEvent(h->stream, st.meas_done, 0));
+    check_obs(h, h->o_kf.p, h->o_lm.p, h->o_w_raw.p, h->El, std::max(h->P, 1), "ccm_ba_create: negative information weight");
+  }
+  apply_edge_flags(h, p->edge_flags != nullptr);
+}
+
+// packed per-pose observation stream for the pose pass
+void pose_obs_stream(ccm_ba_handle* h, const std::vector<int>& udiag, const std::vector<unsigned>& pp) {
+  const int Kf = h->Kf;
+  std::vector<unsigned> kp((size_t)Kf + 1, 0);
+  for (int a = 0; a < Kf; a++) kp[a + 1] = kp[a] + (pp[udiag[a] + 1] - pp[udiag[a]]);
+  upload_vec(h->kobs_ptr, kp, h->stream);
+  h->kobs.alloc(std::max((size_t)kp[Kf], (size_t)1));
+  pack_pose_obs(h);
+}
+
+// landmark-aligned CTA schedule: unit heads (ba_kernels.cuh), numbered by an inclusive scan, cut where a head starts; and the grids
+// of k_linearize and k_backsub_points over it
+void landmark_units(ccm_ba_handle* h) {
+  cudaStream_t s = h->stream;
+  const int Pl = h->Pl;
   h->nunits = 0;
   if (Pl > 0) {
     DevBuf<int> head, rank;
@@ -838,19 +813,22 @@ void build(ccm_ba_handle* h, const ccm_ba_problem* p) {
   } else {
     h->units.alloc_zero(1, s);
   }
-  {
-    int per_sm_lin = 0, per_sm_bs = 0;
-    CCM_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_lin, (const void*)k_linearize, LIN_TILE, 0));
-    CCM_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_bs, (const void*)k_backsub_points, LIN_TILE, 0));
-    h->lin_grid = std::max(1, std::min(h->nunits, sm_count() * std::max(per_sm_lin, 1)));
-    h->bs_grid = std::max(1, std::min(h->nunits, sm_count() * std::max(per_sm_bs, 1)));
-  }
-  // ---- linear-system storage
+  int per_sm_lin = 0, per_sm_bs = 0;
+  CCM_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_lin, (const void*)k_linearize, LIN_TILE, 0));
+  CCM_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm_bs, (const void*)k_backsub_points, LIN_TILE, 0));
+  h->lin_grid = std::max(1, std::min(h->nunits, sm_count() * std::max(per_sm_lin, 1)));
+  h->bs_grid = std::max(1, std::min(h->nunits, sm_count() * std::max(per_sm_bs, 1)));
+}
+
+// linear-system storage and the PCG's shape, then k_pcg2's set-up
+void system_storage(ccm_ba_handle* h, const std::vector<int>& rowptr) {
+  cudaStream_t s = h->stream;
+  const int Kf = h->Kf, Pl = h->Pl, El = h->El, nub = h->nub;
   h->Z.alloc(std::max((size_t)El * 18, (size_t)2));
   h->HllBl.alloc(std::max((size_t)Pl * 9, (size_t)1)); h->gvec.alloc(std::max((size_t)Pl * 3, (size_t)1));
   h->Hbuf.alloc_zero((size_t)Kf * 42 + 2, s);
   h->Ubuf.alloc_zero((size_t)nub * 36 + (size_t)Kf * 6 + 1, s);
-  h->s_val.alloc(std::max<long long>(nnzb * 36, 1)); h->Minv.alloc(std::max((size_t)Kf * 36, (size_t)1));
+  h->s_val.alloc(std::max<long long>(h->nnzb * 36, 1)); h->Minv.alloc(std::max((size_t)Kf * 36, (size_t)1));
   h->bschur.alloc(std::max((size_t)Kf * 6, (size_t)1));
   // coarse space: <= 128 aggregates for small systems, <= 384 for long trajectories where the smooth modes dominate the
   // iteration count; the inverse is refreshed every 2nd solve (measured sweeps: tools/ba_probe.py with CCM_PCG_NC/REFRESH)
@@ -873,31 +851,58 @@ void build(ccm_ba_handle* h, const ccm_ba_problem* p) {
   //   256 / 2: 400, 167.5   320 / 2: 262, 157.1   384 / 2: 212, 160.3
   //   256 / 1: 384, 172.9   320 / 1: 246, 168.7   384 / 1: 197, 179.9
   h->pcg_refresh = std::max(1, env_int("CCM_PCG_REFRESH", 2));
-  setup_pcg2(h, h_rowptr);
+  setup_pcg2(h, rowptr);
   h->partials.alloc((size_t)std::max({sm_count() * 8 + 8, h->lin_grid, h->bs_grid}));
   h->scal.alloc_zero(16, s);
   h->rep_chi2.alloc(std::max(El, 1)); h->rep_depth.alloc(std::max(El, 1));
+}
 
+// the estimate the caller gave, as the current and the trial state
+void initial_state(ccm_ba_handle* h) {
+  cudaStream_t s = h->stream;
   h->pose_cur = h->poseA.p; h->pose_trial = h->poseB.p; h->pt_cur = h->ptA.p; h->pt_trial = h->ptB.p;
-  CCM_CUDA(cudaMemcpyAsync(h->pose_cur, h->pose0.p, h->pose0.bytes(), cudaMemcpyDeviceToDevice, s));
   CCM_CUDA(cudaMemcpyAsync(h->pose_trial, h->pose0.p, h->pose0.bytes(), cudaMemcpyDeviceToDevice, s));
-  if (Pl) CCM_CUDA(cudaMemcpyAsync(h->pt_cur, h->pt0.p, sizeof(double) * 3 * Pl, cudaMemcpyDeviceToDevice, s));
-  if (Pl) CCM_CUDA(cudaMemcpyAsync(h->pt_trial, h->pt0.p, sizeof(double) * 3 * Pl, cudaMemcpyDeviceToDevice, s));
-  h->pose_eval = h->pose_cur; h->pt_eval = h->pt_cur;
-  CCM_CUDA(cudaStreamSynchronize(s));
+  if (h->Pl) CCM_CUDA(cudaMemcpyAsync(h->pt_trial, h->pt0.p, sizeof(double) * 3 * h->Pl, cudaMemcpyDeviceToDevice, s));
+  do_reset(h);
   h->device_bytes = (int64_t)(h->Z.bytes() + h->prod.bytes() + h->s_val.bytes() + h->Ubuf.bytes() +
                               h->bitmap.bytes() + h->word_prefix.bytes() + h->HllBl.bytes() + h->o_kf.bytes() * 2 +
                               h->o_uv.bytes() + h->o_w.bytes() * 2 + h->ptA.bytes() * 3);
-  lap("storage + initial state");
-  h->t_setup_ms = now_ms() - T0;
 }
 
-void do_reset(ccm_ba_handle* h) {
-  cudaStream_t s = h->stream;
-  CCM_CUDA(cudaMemcpyAsync(h->pose_cur, h->pose0.p, h->pose0.bytes(), cudaMemcpyDeviceToDevice, s));
-  if (h->Pl) CCM_CUDA(cudaMemcpyAsync(h->pt_cur, h->pt0.p, sizeof(double) * 3 * h->Pl, cudaMemcpyDeviceToDevice, s));
-  h->pose_eval = h->pose_cur; h->pt_eval = h->pt_cur;
-  CCM_CUDA(cudaStreamSynchronize(s));
+void build(ccm_ba_handle* h, const ccm_ba_problem* p) {
+  const double T0 = now_ms();
+  open_handle(h, p);
+  // CCM_SETUP_PROF=1: wall time of the set-up phases on stderr (each lap synchronises the stream: diagnostics only)
+  const bool sprof = env_int("CCM_SETUP_PROF", 0) != 0;
+  double t_lap = now_ms();
+  auto lap = [&](const char* what) {
+    if (!sprof) return;
+    cudaStreamSynchronize(h->stream);
+    const double t = now_ms();
+    fprintf(stderr, "[ccm_ba_create r%d] %-28s %8.2f ms\n", h->rank, what, t - t_lap);
+    t_lap = t;
+  };
+  Setup st;
+  free_pose_slots(h, p);
+  const ObsLists all = take_observations(h, p, st);
+  map_edge_flags(h, p->edge_flags);   // host work while the measurements are still on their way (one rank)
+  lap("observations + shard");
+  shard_storage(h, p);
+  covisibility_bitmap(h, all, st);
+  lap("points, flags, bitmap, prefix");
+  const Pattern pat = s_pattern(h, st);
+  lap("pattern, upper index");
+  const std::vector<unsigned> pp = product_lists(h, st);
+  schur_schedule(h, pat.udiag, pp);
+  lap("product lists");
+  measurements(h, p, st);
+  pose_obs_stream(h, pat.udiag, pp);
+  lap("pose observation stream");
+  landmark_units(h);
+  system_storage(h, pat.rowptr);
+  initial_state(h);
+  lap("storage + initial state");
+  h->t_setup_ms = now_ms() - T0;
 }
 
 void download_state(ccm_ba_handle* h, ccm_ba_result* r) {
@@ -923,8 +928,7 @@ void download_state(ccm_ba_handle* h, ccm_ba_result* r) {
     h->rep_chi2.download(c.data(), h->El, s); h->rep_depth.download(d.data(), h->El, s);
     CCM_CUDA(cudaStreamSynchronize(s));
     for (int i = 0; i < h->El; i++) {
-      const long long gi = h->E0 + i;
-      const long long e = h->sorted_input ? gi : (long long)h->perm[gi];
+      const long long e = input_edge(h, h->E0 + i);
       if (r->chi2 && !(h->h_flags[i] & 1)) r->chi2[e] = c[i];
       if (r->depth_pos) r->depth_pos[e] = d[i];
     }
@@ -1081,17 +1085,10 @@ extern "C" int ccm_ba_set_edge_flags(ccm_ba_handle* h, const uint8_t* edge_flags
   return guarded([&] {
     CCM_REQUIRE(h, "null handle");
     CCM_CUDA(cudaSetDevice(h->device));
-    for (int i = 0; i < h->El; i++) {
-      const long long gi = h->E0 + i;
-      h->h_flags[i] = edge_flags ? edge_flags[h->sorted_input ? gi : (long long)h->perm[gi]] : 0;
-    }
-    if (h->El) {
-      h->d_flags.upload(h->h_flags.data(), h->El, h->stream);
-      k_apply_flags<<<div_up(h->El, TPB), TPB, 0, h->stream>>>(h->o_w_raw.p, h->d_flags.p, h->El, h->o_w.p);
-      CCM_LAUNCHED();
-      pack_pose_obs(h);
-      CCM_CUDA(cudaStreamSynchronize(h->stream));
-    }
+    map_edge_flags(h, edge_flags);
+    apply_edge_flags(h, edge_flags != nullptr);
+    pack_pose_obs(h);
+    CCM_CUDA(cudaStreamSynchronize(h->stream));
   });
 }
 
@@ -1185,7 +1182,7 @@ extern "C" int ccm_ba_debug_build(ccm_ba_handle* h, int robust, double huber_del
     }
     if (W)
       for (int i = 0; i < El; i++) {
-        const long long e = h->sorted_input ? i : (long long)h->perm[i];
+        const long long e = input_edge(h, i);
         for (int c = 0; c < 18; c++) W[18 * (size_t)e + c] = hW[(size_t)c * h->Ep + i];
       }
     if (chi2_robust_sum) *chi2_robust_sum = hH[(size_t)Kf * 42];

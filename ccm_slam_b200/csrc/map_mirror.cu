@@ -14,7 +14,7 @@
 //       points     alive, not bad, >= min_edges observations in all and >= min_edges selected edges; min_edges = 2 is MapFusionGBA's
 //                  rule (S/Optimizer.cpp:722-740: observations.size() < 2 || nEdges < 2 skips the point), 1 is
 //                  BundleAdjustmentClient's (:117-160: nEdges == 0 removes the vertex); ccm_mirror_set_min_edges, default 2
-//     edges are emitted grouped by point row (counting sort), the order ccm_ba_create's fast path wants;
+//     edges are emitted grouped by point row (counting sort), the order ccm_ba_create takes without grouping on the host;
 //     rows keep first-insertion order (erase + insert again moves to the end), so the result is deterministic — unlike the
 //     reference's, whose edge order follows pointer values (SURVEY.md §7 "hard parts"); BA parity is tolerance-based for that reason.
 // Poses are converted once per SetPose with ccm_pose_from_Tcw_f32 (Converter::toSE3Quat), points widened f32 -> f64 as

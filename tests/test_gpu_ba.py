@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 
 from ccm_slam_b200 import api, synth
+from tests.test_gpu_schur_order import _same_as_grouped
 
 pytestmark = pytest.mark.gpu
 
@@ -60,7 +61,7 @@ def test_lm_matches_oracle_after_same_iteration_count(oracle, name, iters):
     assert np.array_equal(res["depth_pos"], ref["depth_pos"])
 
 
-def test_unsorted_observations_give_the_same_answer(oracle):
+def test_unsorted_observations_give_the_same_answer(oracle, monkeypatch):
     p = synth.make_config("small")
     rng = np.random.default_rng(3)
     perm = rng.permutation(p.E)
@@ -70,6 +71,11 @@ def test_unsorted_observations_give_the_same_answer(oracle):
     b = api.ba_solve(q, iterations=6)
     assert np.allclose(a["poses"], b["poses"], atol=1e-9)
     assert np.allclose(a["chi2"][perm], b["chi2"], rtol=1e-7, atol=1e-9)
+    # against the same observations grouped by a stable sort: lists, system, S, per-edge outputs and state bit-identical through the
+    # permutation, with edge flags given at create and changed by set_edge_flags (bit 0: level 1, bit 1: no robust kernel)
+    monkeypatch.setenv("CCM_PCG_NC", "0")   # read by ccm_ba_create: the coarse level's set-up sums with atomics
+    q.edge_flags = rng.choice(np.arange(4, dtype=np.uint8), p.E, p=[0.7, 0.05, 0.2, 0.05])
+    _same_as_grouped(q, "small", flags=rng.choice(np.arange(4, dtype=np.uint8), p.E, p=[0.6, 0.1, 0.2, 0.1]))
 
 
 def test_create_rejects_bad_observations():

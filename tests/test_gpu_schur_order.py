@@ -81,19 +81,66 @@ def test_product_lists_are_the_pairs_in_landmark_order(name):
         assert np.bincount(blk[:, 0]).max() > 512
 
 
-def _everything(p, lam):
+def _collect(h, lam=1e-3, flags=None):
+    """lists, linear system, S and b_schur at lam, and a 5-iteration state with per-edge chi2 and depth; with flags, another 5
+    iterations from the start after set_edge_flags(flags)"""
+    out = dict(lists=h.debug_products(), build=h.debug_build())
+    out["schur"] = h.debug_schur(lam)
+    out["blocks"] = h.debug_schur_blocks()
+    h.reset()
+    out["final"] = h.optimize(iterations=5, want_edges=True)
+    if flags is not None:
+        h.set_edge_flags(flags)
+        h.reset()
+        out["flagged"] = h.optimize(iterations=5, want_edges=True)
+    for run in ("final", "flagged"):
+        for k in ("t_setup_ms", "t_optimize_ms", "t_download_ms", "t_optimize_event_ms"):
+            out.get(run, {}).pop(k, None)
+    return out
+
+
+def _everything(p, lam=1e-3, flags=None):
     h = api.BAHandle(p)
     try:
-        out = dict(lists=h.debug_products(), build=h.debug_build())
-        out["schur"] = h.debug_schur(lam)
-        out["blocks"] = h.debug_schur_blocks()
-        h.reset()
-        out["final"] = h.optimize(iterations=5)
-        for k in ("t_setup_ms", "t_optimize_ms", "t_download_ms", "t_optimize_event_ms"):
-            out["final"].pop(k)
+        return _collect(h, lam, flags)
     finally:
         h.close()
+
+
+def _shuffled(p, seed):
+    """p with its observations (and edge flags) in random order"""
+    perm = np.random.default_rng(seed).permutation(p.E)
+    q = p.copy()
+    q.obs_kf, q.obs_mp, q.obs_uv, q.obs_w = p.obs_kf[perm], p.obs_mp[perm], p.obs_uv[perm], p.obs_w[perm]
+    q.edge_flags = None if p.edge_flags is None else p.edge_flags[perm]
+    return q
+
+
+def _grouped(q):
+    """q's observations grouped by landmark with a stable sort, as ccm_ba_create groups them, and the permutation that did it"""
+    order = np.argsort(q.obs_mp, kind="stable")
+    g = q.copy()
+    g.obs_kf, g.obs_mp, g.obs_uv, g.obs_w = q.obs_kf[order], q.obs_mp[order], q.obs_uv[order], q.obs_w[order]
+    g.edge_flags = None if q.edge_flags is None else q.edge_flags[order]
+    return g, order
+
+
+def _in_grouped_order(out, order):
+    """_collect's outputs of a create from ungrouped observations, their per-observation arrays (W, chi2, depth) put in grouped order"""
+    out["build"]["W"] = out["build"]["W"][order]
+    for run in ("final", "flagged"):
+        if run in out:
+            out[run]["chi2"] = out[run]["chi2"][order]
+            out[run]["depth_pos"] = out[run]["depth_pos"][order]
     return out
+
+
+def _same_as_grouped(q, label, flags=None):
+    """a create from the ungrouped observations of q against one from the same observations grouped: bit-identical through the
+    permutation (run with the PCG's coarse level off: its set-up sums with atomics); flags in q's order"""
+    g, order = _grouped(q)
+    _same(_everything(g, flags=None if flags is None else flags[order]), _in_grouped_order(_everything(q, flags=flags), order),
+          f"{label} (ungrouped against grouped)")
 
 
 def _same(x, y, path):

@@ -6,8 +6,8 @@ landmark shard, a system of diagonal blocks only), every scene is checked for
   * the product lists against the numpy pairs in landmark order, and the Schur kernel's schedule against its definition;
   * S, b_schur and the landmark step against the f64 restatement of tests/schur_ref.py, entry by entry;
   * Hpp and bp of the pose pass (which reads the diagonal product lists) against tests/ba_ref.py;
-  * bit-identical lists, S, b_schur, Hpp and final state between two creates, with and without the measurement copy on its own
-    stream, after set_estimate against a fresh create at that state, and after reset.
+  * bit-identical lists, S, b_schur, Hpp and final state between two creates, between the observations in shuffled order and
+    grouped, after set_estimate against a fresh create at that state, and after reset.
 The loop-closure scene also runs LM against the oracle."""
 import numpy as np
 import pytest
@@ -17,7 +17,7 @@ from tests import ba_ref as F
 from tests import schur_ref as R
 from tests import schur_setup_scenes as SC
 from tests.test_gpu_ba import _state_close
-from tests.test_gpu_schur_order import _expected, _same
+from tests.test_gpu_schur_order import _collect, _everything, _expected, _same, _same_as_grouped, _shuffled
 
 pytestmark = pytest.mark.gpu
 
@@ -195,39 +195,18 @@ def test_pose_pass_matches_the_restatement(dev, name, robust, capsys):
         assert v <= 1.0, f"{name} robust={robust}: {k} of pose {at} at err/tol {v:.3g}"
 
 
-def _collect(h, lam=1e-3):
-    out = dict(lists=h.debug_products(), build=h.debug_build())
-    out["schur"] = h.debug_schur(lam)
-    out["blocks"] = h.debug_schur_blocks()
-    h.reset()
-    out["final"] = h.optimize(iterations=5)
-    for k in ("t_setup_ms", "t_optimize_ms", "t_download_ms", "t_optimize_event_ms"):
-        out["final"].pop(k)
-    return out
-
-
-def _fresh(p, overlap, monkeypatch):
-    monkeypatch.setenv("CCM_MEAS_OVERLAP", str(overlap))   # read by ccm_ba_create
-    h = api.BAHandle(p)
-    try:
-        return _collect(h)
-    finally:
-        h.close()
-
-
 @pytest.mark.parametrize("name", NAMES)
 def test_setup_is_deterministic(dev, name, monkeypatch):
-    """two creates, a create without and one with the measurement copy on its own stream, a handle moved by set_estimate against a
-    fresh create at that state, and a second pass after reset: bit-identical lists, S, b_schur, Hpp and 5-iteration state"""
+    """two creates, the same observations in shuffled order against them grouped, a handle moved by set_estimate against a fresh
+    create at that state, and a second pass after reset: bit-identical lists, S, b_schur, Hpp and 5-iteration state"""
     monkeypatch.setenv("CCM_PCG_NC", "0")   # read by ccm_ba_create: the coarse level's set-up sums with atomics
     p = scene(name)
-    first = _fresh(p, 1, monkeypatch)
-    _same(first, _fresh(p, 1, monkeypatch), f"{name} (two creates)")
-    _same(first, _fresh(p, 0, monkeypatch), f"{name} (CCM_MEAS_OVERLAP 0 and 1)")
+    first = _everything(p)
+    _same(first, _everything(p), f"{name} (two creates)")
+    _same_as_grouped(_shuffled(p, 11), name)
     q = p.copy()
     q.poses[:, 4:] += 1e-3
     q.points = q.points + 1e-3
-    monkeypatch.setenv("CCM_MEAS_OVERLAP", "1")
     h = api.BAHandle(p)
     try:
         h.debug_schur(1e-3)
@@ -237,7 +216,7 @@ def test_setup_is_deterministic(dev, name, monkeypatch):
         again = _collect(h)
     finally:
         h.close()
-    _same(moved, _fresh(q, 1, monkeypatch), f"{name} (set_estimate against a fresh create)")
+    _same(moved, _everything(q), f"{name} (set_estimate against a fresh create)")
     _same(moved, again, f"{name} (after reset)")
 
 
